@@ -489,7 +489,7 @@ def RunBenchmark(args, clock_sampler_cls):
                    'parallelism': 'dp%d+ep%d' % (world, min(world, cfg.experts)),
                    'experts': cfg.experts, 'model_dim': cfg.model_dim,
                    'layers': cfg.layers, 'optimizer': 'Adafactor (unfused torch ops)',
-                   'l2_flush': 'working set (1.4B fp32 params + activations) >> 126 MB '
+                   'l2_flush': 'working set (1.4B fp32 params + activations) >> 50 MB '
                                'L2; no explicit flush'},
         'clocks': clocks.Summary(),
         'exposed_a2a_ms_per_step': float(a2a.item()),

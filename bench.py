@@ -48,6 +48,10 @@ def _ParseArgs():
   ap.add_argument('--cuda-graph', default='auto', choices=['auto', 'on', 'off'],
                   help='Capture the whole train step into a CUDA graph (auto: fall back '
                   'to eager launches if capture fails).')
+  ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                  help='After the timed steps, write what the last timed step returned '
+                  '(metrics, per-example outputs) and a fixed sample of the updated '
+                  'weights as DIR/<name>.npy.')
   return ap.parse_args()
 
 
@@ -145,9 +149,15 @@ def main():
   if args.comm:
     os.environ['LINGVO_B200_COMM'] = args.comm
 
+  import random
   import tempfile
+  import numpy as np
   import torch
   import torch.distributed as dist
+  # Weight init and the synthetic batches draw from these: same arguments, same inputs.
+  random.seed(0)
+  np.random.seed(0)
+  torch.manual_seed(0)
   world = int(os.environ.get('WORLD_SIZE', '1'))
   rank = int(os.environ.get('RANK', '0'))
   local_rank = int(os.environ.get('LOCAL_RANK', '0'))
@@ -194,17 +204,22 @@ def main():
         sync()
         e0.record()
         for i in range(n_steps):
-          m, _ = engine.Step(batches[(n_warm + i) % len(batches)])
+          m, per_example = engine.Step(batches[(n_warm + i) % len(batches)])
         e1.record()
         sync()
       ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
       if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
-      return float(ms.item()), m
+      return float(ms.item()), m, per_example
 
+    # CUDA-graph capture (it runs warm-up steps of its own) happens here, never inside the
+    # timed window, so the window holds exactly --steps train steps.
+    engine._MaybeCapture(batches[0])   # pylint: disable=protected-access
     launches0 = native.launch_count()
     clocks = ClockSampler(local_rank)
-    ms_total, metrics = timed(args.warmup, args.steps, clocks)
+    ms_total, metrics, per_example = timed(args.warmup, args.steps, clocks)
+    if args.dump_outputs and rank == 0:
+      _DumpOutputs(args.dump_outputs, metrics, per_example, task)
     launches = native.launch_count() - launches0
     if engine.cuda_graph:
       # kernels of ours executed per replay (counted while capturing) × timed steps
@@ -263,8 +278,8 @@ def main():
             'experts': tp.builder.e_dim, 'model_dim': tp.builder.model_dim,
             'layers': tp.num_transformer_layers,
             'optimizer': type(task.learners[0].optimizer).__name__,
-            'l2_flush': 'working set (1.4B fp32 params + bf16 activations) '
-                        'is >> 126 MB L2; no explicit flush',
+            'l2_flush': 'working set (fp32 params + bf16 activations) '
+                        'is >> 50 MB L2; no explicit flush',
         },
         'clocks': clocks.Summary(), 'gpu_launches': int(launches),
         'final_loss': loss,
@@ -296,6 +311,47 @@ def main():
   return 0
 
 
+_DUMP_LIMIT_BYTES = 64 << 20
+_WEIGHT_SAMPLE = 4096
+
+
+def _DumpOutputs(out_dir, metrics, per_example, task):
+  """Writes the last timed step's results as float32/float64 `.npy` files: every metric
+  (value and weight), every per-example output, and for each weight the same seeded sample
+  of at most `_WEIGHT_SAMPLE` elements after the update."""
+  import numpy as np
+  import torch
+  os.makedirs(out_dir, exist_ok=True)
+  arrays = {}
+
+  def _Add(name, v):
+    t = torch.as_tensor(v).detach()
+    dtype = torch.float64 if t.dtype == torch.float64 else torch.float32
+    arrays[name] = t.to(dtype).cpu().numpy()
+
+  for k, v in sorted(metrics.items()):
+    if isinstance(v, (tuple, list)):
+      _Add('metric.%s' % k, v[0])
+      _Add('metric.%s.weight' % k, v[1])
+    else:
+      _Add('metric.%s' % k, v)
+  if per_example:
+    for k, v in per_example.FlattenItems():
+      if isinstance(v, torch.Tensor) or np.isscalar(v):
+        _Add('per_example.%s' % k, v)
+  for k, v in task.vars.FlattenItems():
+    flat = v.detach().reshape(-1)
+    if flat.numel() > _WEIGHT_SAMPLE:
+      gen = torch.Generator().manual_seed(0)
+      idx = torch.randperm(flat.numel(), generator=gen)[:_WEIGHT_SAMPLE].sort().values
+      flat = flat[idx.to(flat.device)]
+    _Add('weight.%s' % k, flat)
+  total = sum(a.nbytes for a in arrays.values())
+  assert total <= _DUMP_LIMIT_BYTES, 'dump of %d bytes exceeds 64 MB' % total
+  for k, a in arrays.items():
+    np.save(os.path.join(out_dir, k.replace('/', '.') + '.npy'), a)
+
+
 class _Null:
 
   def __enter__(self):
@@ -322,7 +378,7 @@ def _ExposedA2A(task, engine, batches, ms_normal, timed, args):
       ex.loopback = True
     if saved is not None:
       engine._graphed = graph_step.GraphedTrainStep(task, batches[0], warmup=2)  # pylint: disable=protected-access
-    ms_lb, _ = timed(2, args.steps)
+    ms_lb = timed(2, args.steps)[0]
     return max(0.0, ms_normal - ms_lb / args.steps)
   except Exception as e:  # pylint: disable=broad-except
     sys.stderr.write('exposed-a2a measurement failed: %r\n' % (e,))

@@ -6,7 +6,7 @@ Reference `lingvo/core/base_input_generator.py`: `BaseInputGenerator` params
 (:1223-1296), sequence generators (:1465-1697), `BaseTinyDatasetInput`
 (:1706-1767).
 
-B200-first: a batch is a NestedMap of **pinned host tensors** produced by
+H100-first: a batch is a NestedMap of **pinned host tensors** produced by
 native C++ threads (`lingvo_b200.ops.native_input`); `DevicePrefetcher`
 overlaps the H2D copy of batch i+1 with the compute of batch i on a side
 stream — the analogue of the reference's TPU infeed queues.

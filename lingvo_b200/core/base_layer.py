@@ -148,7 +148,7 @@ class BaseLayer(metaclass=BaseLayerMeta):
     p.Define('name', '', 'Name of this layer object, must be a valid id.')
     p.Define('dtype', torch.float32, 'Datatype of the variables.')
     p.Define('fprop_dtype', None,
-             'Activations datatype; None ⇒ same as dtype. bf16 is the B200 '
+             'Activations datatype; None ⇒ same as dtype. bf16 is the H100 '
              'tensor-core path.')
     p.Define('random_seed', None,
              'Layer-local random seed. None ⇒ non-deterministic init; set ⇒ '

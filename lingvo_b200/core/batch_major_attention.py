@@ -7,14 +7,14 @@ MultiHeadedProjectionLayer, :481 MultiHeadedAttention, :2233 …XL, :2413 …RPE
 TransformerAttentionLayer, :6265 TransformerLayer, :7116
 StackedTransformerLayers, :8591 Builder).
 
-B200-first design choices (not a translation):
+H100-first design choices (not a translation):
   * Every mask (padding, causal, per-step, segment, local band, chunk) and every
     relative-position term (XL, RPE) is folded into ONE additive bias and the
     core runs through `ops.attention.dot_product_attention`, whose CUDA path is
     a fused online-softmax kernel — the `[B,N,T,S]` logits are only
     materialised when the caller asks for probabilities.
   * Projections `[D, N, H]` are stored exactly like the reference (checkpoint
-    parity) and run as flat `[D, N·H]` tcgen05 GEMMs with fused bias.
+    parity) and run as flat `[D, N·H]` wgmma GEMMs with fused bias.
   * Decode caches are `[T, B, N, H]` like the reference's `InitStates`.
 """
 

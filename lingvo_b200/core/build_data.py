@@ -12,5 +12,5 @@ def BuildData():
   p.Define('torch_version', torch.__version__, 'PyTorch version.')
   p.Define('cuda_version', str(torch.version.cuda), 'CUDA runtime version.')
   p.Define('python_version', platform.python_version(), 'Python version.')
-  p.Define('target_arch', 'sm_100a', 'GPU architecture the native kernels are built for.')
+  p.Define('target_arch', 'sm_90a', 'GPU architecture the native kernels are built for.')
   return p

@@ -27,7 +27,7 @@ class Base:
     p = hyperparams.InstantiableParams(cls)
     p.Define('deterministic_dropout', False, 'Use deterministic dropout.')
     p.Define('dtype', torch.float32, 'Variable dtype.')
-    p.Define('fprop_dtype', None, 'Activations dtype (bf16 on B200).')
+    p.Define('fprop_dtype', None, 'Activations dtype (bf16 on H100).')
     p.Define('device_mesh', None, 'np.ndarray device mesh.')
     p.Define('weight_split_dims_mapping', None, 'Default weight sharding.')
     p.Define('activation_split_dims_mapping', None, 'Default act sharding.')

@@ -4,7 +4,7 @@ Reference: `lingvo/core/cluster.py` — `_Cluster.Params()` job specs (:72-169),
 derived quantities (:377-515), variable placers (:586-654), thread-local
 cluster stack (:66,254-265).
 
-B200-first re-design: there is ONE process per GPU (torchrun). A "replica" is
+H100-first re-design: there is ONE process per GPU (torchrun). A "replica" is
 a rank; `worker.replicas × worker.gpus_per_replica` therefore equals the
 world size of the data-parallel group when launched distributed, and the
 parameter-server job disappears: `VarPlacer` becomes the *optimizer-state
@@ -49,7 +49,7 @@ def _JobSpec(replicas: int, name: str = ''):
   p.Define('targets', '', 'Comma-separated host:port rendezvous targets.')
   p.Define('cpus_per_replica', 1, 'CPU devices per replica.')
   p.Define('gpus_per_replica', 0, 'GPUs per replica.')
-  p.Define('tpus_per_replica', 0, 'Kept for parity; always 0 on B200.')
+  p.Define('tpus_per_replica', 0, 'Kept for parity; always 0 on H100.')
   p.Define('devices_per_split', 1, 'Devices one model split spans.')
   p.Define('num_tpu_hosts', 0, 'Kept for parity.')
   p.Define('additional_worker_names', [], 'Kept for parity.')

@@ -5,7 +5,7 @@ BN/GroupNorm/LN → Swish → linear → dropout → +residual.
 `ConformerLayer` (ref :471): ½·FFN → MHSA / LConv (order configurable) →
 ½·FFN → final LN, with streaming (`StreamStep`) for causal configs.
 
-B200 path of the conv module: the three memory-bound stages in the middle
+H100 path of the conv module: the three memory-bound stages in the middle
 (GLU gate, padding mask, depthwise conv) run as ONE kernel
 (`ops.conv.glu_dwconv1d`) that reads the `[B,T,2D]` projection once and writes
 `[B,T,D]` once; LN/GroupNorm + Swish follow in the fused norm kernel.

@@ -8,7 +8,7 @@ padding is the max-pool of the input padding over the conv window (ref :76,
 and support `StreamStep` with a `(k−1)·dilation`-frame rolling context.
 
 NHWC activations are kept as-is (channels-last is what cuDNN/our depthwise
-kernel want on B200); weights keep the reference's `[h, w, in, out]` layout.
+kernel want on H100); weights keep the reference's `[h, w, in, out]` layout.
 """
 
 from __future__ import annotations

@@ -20,7 +20,7 @@ reference:
     `statistics_computation_frequency` thins the statistics updates, `exponent_multiplier`
     scales the inverse-root exponent.
 
-B200 design. The statistics updates are `tensordot`s — GEMMs on the tensor cores, fp32
+H100 design. The statistics updates are `tensordot`s — GEMMs on the tensor cores, fp32
 accumulate. The inverse p-th roots are the only super-linear part; they run every
 `preconditioning_compute_steps`:
   * synchronously with the coupled Newton iteration of `matrix_functions` (all matmuls), or

@@ -8,7 +8,7 @@
   pipeline stage i over `num_micro_batches` micro-batches.
 
 The reference pipelines inside one TF graph with `recurrent.StackedRecurrent`
-(Send/Recv between devices of one process). On B200 each GPU is its own
+(Send/Recv between devices of one process). On H100 each GPU is its own
 process, so stages live on different ranks and activations/gradients move as
 NCCL point-to-point transfers over NVLink — that engine is
 `lingvo_b200.parallel.pp.PipelineEngine`. When all stages are in this process

@@ -1,7 +1,7 @@
 """CUDA-graph capture of a whole training step.
 
-The train step of a large model issues ~2000 kernel launches from Python; on B200 the GPU
-finishes them faster than the host can enqueue them. `GraphedTrainStep` captures
+The train step of a large model issues hundreds of kernel launches from Python, and the host
+loop that enqueues them can become the critical path. `GraphedTrainStep` captures
 FProp → BProp → gradient sync → optimizer of a task ONCE into a CUDA graph and replays it:
 one launch per step, the host only refreshes the inputs and the two step-dependent
 hyper-parameters (learning rate, Adafactor decay), which live in device memory.

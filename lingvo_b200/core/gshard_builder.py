@@ -11,8 +11,8 @@ FFN (`DenseReluDense :2939`, gated :3054), MoE (`MoE :2465`,
 
 Re-design: the reference composes every block from a string-signature graph
 DSL and relies on XLA to fuse/shard it. Here each block is an explicit layer
-class whose `FProp` calls the fused sm_100a kernels directly (RMS-norm,
-tcgen05 GEMM w/ fused epilogues, index-based MoE dispatch/combine, fused
+class whose `FProp` calls the fused sm_90a kernels directly (RMS-norm,
+wgmma GEMM w/ fused epilogues, index-based MoE dispatch/combine, fused
 xent), and whose collectives are explicit (`lingvo_b200.parallel`). The
 builder API (method names, params, sub-layer type lists) is kept so
 experiment configs port 1:1.
@@ -187,11 +187,8 @@ class RmsNormLayer(_BuilderLayer):
 
 
 class _EmbedRows(torch.autograd.Function):
-  """out[i] = w[ids[i]]; d_w = scatter-add of d_out rows, accumulated in fp32.
-
-  The stock `embedding_dense_backward` sorts the ids and runs a segmented reduction
-  (≈0.6 ms for 8k tokens × 2048 on a B200); an atomics scatter into an fp32 staging table
-  is several times faster and at least as accurate (fp32 accumulation of duplicate tokens)."""
+  """out[i] = w[ids[i]]; d_w = sum of d_out rows per id, accumulated in fp32 in a fixed
+  (sorted-index) order, so duplicate tokens give the same gradient on every run."""
 
   @staticmethod
   def forward(ctx, w, ids):
@@ -204,7 +201,9 @@ class _EmbedRows(torch.autograd.Function):
   def backward(ctx, dy):
     (flat,) = ctx.saved_tensors
     dw = torch.zeros(ctx.w_shape, dtype=torch.float32, device=dy.device)
-    dw.index_add_(0, flat, dy.reshape(-1, dy.shape[-1]).float())
+    # index_put_(accumulate=True) sorts the indices on CUDA: duplicate ids are summed in a
+    # fixed order, so the gradient is the same on every run (index_add_ uses atomics).
+    dw.index_put_((flat,), dy.reshape(-1, dy.shape[-1]).float(), accumulate=True)
     return dw.to(ctx.w_dtype), None
 
 
@@ -268,9 +267,10 @@ class _BucketGather(torch.autograd.Function):
   @staticmethod
   def backward(ctx, dt):
     (bucket,) = ctx.saved_tensors
-    dw = torch.zeros(dt.shape[0], ctx.nb, dtype=dt.dtype, device=dt.device)
-    dw.index_add_(1, bucket, dt.contiguous())
-    return dw, None
+    # Summed in a fixed order (sorted indices), unlike index_add_'s atomics.
+    dw = torch.zeros(ctx.nb, dt.shape[0], dtype=dt.dtype, device=dt.device)
+    dw.index_put_((bucket,), dt.t(), accumulate=True)
+    return dw.t(), None
 
 
 class SelfAttentionLayer(_BuilderLayer):
@@ -384,8 +384,8 @@ class SelfAttentionLayer(_BuilderLayer):
         rel, b.relative_attention_num_buckets,
         b.relative_attention_max_distance, bidirectional=bidi)
     if theta.wrb.is_cuda:
-      # gather forward, atomic index_add backward (a few µs each; the one-hot fp32 matmul
-      # this replaces ran as a 50 µs SIMT sgemm per layer and direction).
+      # gather forward, sorted index_put_ backward: replaces a one-hot fp32 matmul per layer
+      # and direction.
       return _BucketGather.apply(theta.wrb.float(), bucket.long())
     onehot = F.one_hot(bucket.long(), b.relative_attention_num_buckets).float()
     return torch.matmul(theta.wrb.float(), onehot.t())
@@ -490,7 +490,7 @@ class SelfAttentionLayer(_BuilderLayer):
     if simple and toeplitz and hk == h:
       from lingvo_b200.ops import attention as attention_ops
       if attention_ops.flash_attention_supported(q, k, drop):
-        # Our tcgen05 flash attention: bias table + packed-input mask applied in registers,
+        # Our wgmma flash attention: bias table + packed-input mask applied in registers,
         # dRel folded into the backward; output already `[B, L, H, D]`.
         rel = self._RelTable(theta, l, x.device) if self.params.relative_bias else None
         causal = self.params.decoder and not b.decoder_skip_causal_mask
@@ -502,7 +502,7 @@ class SelfAttentionLayer(_BuilderLayer):
       from lingvo_b200.ops import attention as attention_ops
       rel = self._RelTable(theta, l, x.device)
       if attention_ops.rel_bias_attention_supported(q, k, rel, drop):
-        # cuDNN fused attention + our bias-build / tcgen05 bias-gradient kernels.
+        # cuDNN fused attention + our bias-build / wgmma bias-gradient kernels.
         mask = self._Mask(segment_id, segment_pos, torch.float32)
         o = attention_ops.rel_bias_attention(
             q, k, v, rel, mask, 1.0,
@@ -901,7 +901,7 @@ class MoELayer(_BuilderLayer):
   Variables: `top_2_gating.w [M, E]`, `wi [E(_local), M, H]`,
   `wo [E(_local), H, M]` (GLU: `wi_0/wi_1`). Tokens `[B, L, M]` are grouped
   to `[G, S, M]`, gated (fp32 logits), dispatched to experts, and combined.
-  `mode`: 'indexed' (B200 path) or 'dense' (reference einsum oracle).
+  `mode`: 'indexed' (H100 path) or 'dense' (reference einsum oracle).
   """
 
   @classmethod
@@ -1281,7 +1281,7 @@ class MoEBuilder(builder.Base):
     p.Define('scale_input_embedding_by_dim', False, 'Scale embeddings.')
     p.Define('softplus_scale_q', False, 'Kept for parity.')
     p.Define('ff_use_bias', False, 'Bias in dense FFN.')
-    p.Define('moe_mode', 'indexed', 'indexed (fused B200 path) | dense oracle.')
+    p.Define('moe_mode', 'indexed', 'indexed (fused H100 path) | dense oracle.')
     p.Define('remat', False, 'Rematerialise blocks in backward.')
     p.Define('context_parallel', False,
              'Shard the *sequence* dimension over the ranks (context parallelism, '
@@ -1550,7 +1550,7 @@ RecurrentDenseBuilder = DenseBuilder
 class RecurrentDenseBuilderParallelDecode(DenseBuilder):
   """`DenseBuilder` whose projection weights are split into *micro variables* of shape
   `[model_dim, proj_weight_hdim, d_kv]` (reference :3478) so that no single variable of a
-  very deep repeated stack exceeds one host's memory. On B200 the 180 GB of HBM hold the
+  very deep repeated stack exceeds one host's memory. On H100 the 80 GB of HBM hold the
   fused `[M, H·D]` weights directly and the kernels want them contiguous, so the weights
   stay fused; the class keeps the knob (checkpoint converters use it to split / merge the
   micro variables) and forces deterministic dropout like the reference."""

@@ -2,7 +2,7 @@
 
 The reference keeps a TPU program spinning in an infinite `while_loop`, feeding it
 through infeed queues from a host thread and draining results through outfeed. The
-B200 design keeps the same three-stage shape with CUDA streams instead of TPU
+H100 design keeps the same three-stage shape with CUDA streams instead of TPU
 queues:
 
   infeed thread  : host batches → pinned buffers → H2D on a copy stream

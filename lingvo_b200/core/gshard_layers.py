@@ -4,7 +4,7 @@ Reference `lingvo/core/gshard_layers.py`:
   * `Top2GatingOnLogits` (:1932-2364) — reproduced verbatim in *math* as the
     dense `GSEC` oracle (`Top2GatingOnLogits`), and re-designed as an
     **index-based** gate (`Top2GatingIndices`) that returns
-    `(expert, slot, gate) × 2` per token — what the fused sm_100a gate kernel
+    `(expert, slot, gate) × 2` per token — what the fused sm_90a gate kernel
     (`ops.moe.top2_gate`) produces. Both implement: softmax over E, top-1,
     second-expert policy (`all` / `sampling` (Gumbel) / `random` threshold),
     exclusive cumsum positions with first-choice priority (:2230, :2294),
@@ -13,8 +13,8 @@ Reference `lingvo/core/gshard_layers.py`:
     (:2250-2255).
   * `ComputeGating` (:2840-2964), `FeedForwardNetworksApplyGating`
     (:2992-3163) — dense einsum oracle `GSEC,GSM->EGCM` … `GSEC,GECM->GSM`.
-  * `MoEApplyIndexed` — the B200 path: permute-scatter dispatch, grouped
-    tcgen05 expert GEMMs, gated 2-row gather combine; with expert parallelism
+  * `MoEApplyIndexed` — the H100 path: permute-scatter dispatch, grouped
+    wgmma expert GEMMs, gated 2-row gather combine; with expert parallelism
     the scatter/gather cross NVLink (`lingvo_b200.parallel.ep`).
   * `HashGatingOnLogits` (:2367), `TokenShufflingOnlogits` (:2496),
     sentence/task-level gating (:3359, :3450), `ReshapeInputLayer` (:1614),

@@ -4,7 +4,7 @@ Reference `lingvo/core/gshard_utils.py`: `Split/Replicate/MeshSplit` (:40-134)
 annotate tensors and XLA's SPMD partitioner inserts the collectives — and
 every annotation is a no-op off-TPU. Here an annotation *records* a
 `TensorShardingSpec` on the tensor (`tensor._sharding`) which the explicit
-B200 runtime (`lingvo_b200.parallel`) reads: layers that own a collective
+H100 runtime (`lingvo_b200.parallel`) reads: layers that own a collective
 (MoE all-to-all, TP GEMM+reduce-scatter, vocab-sharded softmax) query the
 active `parallel.mesh.DeviceMesh` and run their fused kernels; everything else
 stays local. `TensorShardingSpec` keeps the reference's uneven-padding

@@ -1,7 +1,7 @@
 """Inference export (ref `lingvo/core/inference_graph_exporter.py`).
 
 The reference freezes a TF `GraphDef` plus `subgraphs{name: feeds, fetches}`. The
-B200 equivalent of "a frozen graph" is a self-contained **inference bundle**:
+H100 equivalent of "a frozen graph" is a self-contained **inference bundle**:
 
   <dir>/inference_graph.json   model name, task, subgraph names + their feed/fetch
                                keys, dtype policy, bundle format version

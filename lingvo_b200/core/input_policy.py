@@ -1,7 +1,7 @@
 """Input placement policy (ref `lingvo/core/input_policy.py`).
 
 `Apply(input_params)` returns params of a subclass of the input generator that is pinned to
-the cluster's *input device* — the host on a B200 box: batches are assembled (and split for
+the cluster's *input device* — the host on a H100 box: batches are assembled (and split for
 towers) in host memory, ideally pinned, and only the `DevicePrefetcher` of the train engine
 moves them to the GPU with an asynchronous copy that overlaps the previous step. Without the
 policy an input generator written with device-agnostic factory calls could allocate on

@@ -3,8 +3,8 @@
 Catalogue follows reference `lingvo/core/layers.py` (63 classes, SURVEY §2.4).
 Activations are NHWC / `[batch, time, …, channels]` like the reference;
 `paddings` are `[batch, time]` floats (1 = padded). Each layer cites the
-reference line it mirrors. Compute is PyTorch with the sm_100a kernels
-(`lingvo_b200.ops`: tcgen05 GEMM with fused bias/activation, fused
+reference line it mirrors. Compute is PyTorch with the sm_90a kernels
+(`lingvo_b200.ops`: wgmma GEMM with fused bias/activation, fused
 LayerNorm, fused softmax-xent) swapped in on CUDA bf16 paths.
 """
 
@@ -398,7 +398,7 @@ class Conv2DLayerNoPadding(base_layer.BaseLayer):
 class ProjectionLayer(quant_utils.QuantizableLayer):
   """y = act(BN(x·w + b)) (reference :845-1417).
 
-  On CUDA/bf16 without BN the GEMM + bias + activation run as ONE tcgen05
+  On CUDA/bf16 without BN the GEMM + bias + activation run as ONE wgmma
   kernel (`ops.gemm.linear`).
   """
 
@@ -1854,7 +1854,7 @@ class LayerNorm(base_layer.BaseLayer):
   """Layer normalisation (reference :4927).
 
   scale stored as `(1 + scale)` unless `direct_scale`; `bias`/`center`
-  switches. On CUDA the fused sm_100a kernel (`ops.norm.layer_norm`) is used.
+  switches. On CUDA the fused sm_90a kernel (`ops.norm.layer_norm`) is used.
   """
 
   @classmethod

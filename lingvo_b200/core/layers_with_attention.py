@@ -536,7 +536,7 @@ class TransformerShardedMoeLayer(base_layer.BaseLayer):
   `py_utils.AuxLossContext`. Expert weights `wi_<k> [E, D, H/shards]`, `wo_<k>`.
 
   On a GPU, with bf16 activations, ReLU experts and top-2 gating, the expert path is the
-  fused peer-memory exchange of `parallel/symm.py` (gate+dispatch kernel, grouped tcgen05
+  fused peer-memory exchange of `parallel/symm.py` (gate+dispatch kernel, grouped wgmma
   GEMMs, row-pointer combine); otherwise the index-dispatch reference path.
   """
 

@@ -5,7 +5,7 @@ Contract per reference `lingvo/core/learner.py` (`Apply` :177-239,
 :353-500 — L1/L2 via gradient adjust, global-norm clip, clip-to-zero,
 NaN/Inf ⇒ grad_scale = 0 step skip — and eval metrics :170-175, :462-495).
 
-B200-first: gradients come from autograd. When the task's data-parallel
+H100-first: gradients come from autograd. When the task's data-parallel
 engine (`parallel/dp.py`) owns the variables, the engine's bucketed
 reduce-scatter / fused scale+Adam path is invoked through
 `self.grad_sync`, and the scalar bookkeeping (norms, NaN check) is done on

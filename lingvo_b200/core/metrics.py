@@ -3,7 +3,7 @@
 `BaseMetric` / `AverageMetric` / `F1Metric` / `MCCMetric` / `CorpusBleuMetric`
 / `AUCMetric` / `CorrelationMetric` / `SamplingMetric` / `MultiClassAUCMetric`
 / `AverageKeyedCustomMetric` and a device-side accumulator
-(`DeviceEvalMetrics`, the B200 analogue of `TpuEvalMetrics` :258-384: metric
+(`DeviceEvalMetrics`, the H100 analogue of `TpuEvalMetrics` :258-384: metric
 (value, weight) pairs are accumulated on the GPU across loop steps and only
 synced to host once per eval program).
 """

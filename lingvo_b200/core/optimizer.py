@@ -6,11 +6,11 @@ Catalogue and update rules follow reference `lingvo/core/optimizer.py`
 :507, `DynamicAccumulator` :575, `DistributedShampoo` :689, `AdaGraft` :803,
 `XLAShardingAdafactor` :905-1275, `GradientAggregationOptimizer` :1276).
 
-B200-first design: an optimizer is a layer owning *slot tensors* keyed by the
+H100-first design: an optimizer is a layer owning *slot tensors* keyed by the
 variable's checkpoint name (`<var>/Adam`, `<var>/Adam_1`, …, the TF names, so
 checkpoints keep the reference layout). `Apply(lr, var_grads)` updates the
 Parameters in place under `no_grad`; on CUDA the dense rules run as
-multi-tensor (`torch._foreach_*`) launches or as the fused sm_100a kernels in
+multi-tensor (`torch._foreach_*`) launches or as the fused sm_90a kernels in
 `lingvo_b200.ops.optim` (Adam / Adafactor), and the data-parallel runtime
 (`parallel/dp.py`) fuses reduce-scatter + the same Adam math over a flat shard.
 """
@@ -360,7 +360,7 @@ class Adam(Base):
     p.Define('beta1', 0.9, 'Beta1 for Adam.')
     p.Define('beta2', 0.999, 'Beta2 for Adam.')
     p.Define('epsilon', 1e-6, 'Epsilon for Adam.')
-    p.Define('fused', True, 'Use the fused sm_100a multi-tensor kernel on CUDA.')
+    p.Define('fused', True, 'Use the fused sm_90a multi-tensor kernel on CUDA.')
     return p
 
   @classmethod
@@ -500,7 +500,7 @@ class GradientAggregation(Base):
 
   Grads of `num_micro_batches` consecutive Apply calls are summed locally; the
   all-reduce (via `reduce_fn`) happens once, right before the wrapped
-  optimizer's apply — the B200 analogue of `GradientAggregationOptimizer`.
+  optimizer's apply — the H100 analogue of `GradientAggregationOptimizer`.
   """
 
   SLOT_SUFFIX = {'grad_accum': 'grad_accum'}
@@ -585,7 +585,7 @@ class XLAShardingAdafactor(Base):
     p.Define('cond_is_finite', False, 'Skip the update if stats are not finite.')
     p.Define('epsilon1', 1e-30, 'Regularization constant for squared gradient.')
     p.Define('epsilon2', 1e-3, 'Regularization constant for parameter scale.')
-    p.Define('fused', True, 'Use the fused sm_100a kernel on CUDA.')
+    p.Define('fused', True, 'Use the fused sm_90a kernel on CUDA.')
     p.Define('num_update_streams', 8,
              'Factored variables are spread round-robin over this many CUDA streams, so that '
              'the latency-bound kernels of small tensors overlap (also inside a captured '
@@ -662,6 +662,15 @@ class XLAShardingAdafactor(Base):
             sorted(dims) == [var.dim() - 2, var.dim() - 1] and var.shape[-1] % 8 == 0 and
             var.is_contiguous())
 
+  def _SlotIndex(self, idx, device):
+    """Device index tensor of `idx`, built once per variable set: the first (eager) steps
+    create it, so a captured step never copies it from the host."""
+    cache = self.__dict__.setdefault('_slot_index_cache', {})
+    key = (tuple(idx), str(device))
+    if key not in cache:
+      cache[key] = torch.tensor(idx, dtype=torch.long, device=device)
+    return cache[key]
+
   def PreGradStats(self, var_grad_pairs):
     """Phase A of the fused step for every eligible variable. The same pass that builds the
     factored second-moment sums also yields Σg² — the learner gets the global gradient
@@ -685,7 +694,11 @@ class XLAShardingAdafactor(Base):
     self._pre_var_sumsq = None
     self._pre_ep_sumsq = None
     fan = self._UpdateFan(total.device)
-    for var, grad in var_grad_pairs:
+    # One Σg² slot per variable (the stats kernels of different side streams never share an
+    # accumulator), summed below in variable order: the norm is the same on every run.
+    parts = torch.zeros(len(var_grad_pairs), dtype=torch.float32, device=total.device)
+    dense_idx, ep_idx = [], []
+    for k, (var, grad) in enumerate(var_grad_pairs):
       dims = self._FactoredDims(list(var.shape))
       if grad.device == var.device and self._SmallEligible(var, grad, dims):
         small.append((var, grad))
@@ -697,10 +710,15 @@ class XLAShardingAdafactor(Base):
       with fan.On(len(handled)):
         fresh = fused.adafactor_stats(var, grad, dims[0], dims[1],
                                       bool(p.multiply_by_parameter_scale),
-                                      total_ep if is_ep else total, fan.Slot(len(handled)))
+                                      parts[k:k + 1], fan.Slot(len(handled)))
+      (ep_idx if is_ep else dense_idx).append(k)
       self._pre[id(var)] = (grad.data_ptr(), fresh)
       handled.add(id(var))
     fan.Join()
+    if dense_idx:
+      total = total + parts.index_select(0, self._SlotIndex(dense_idx, parts.device)).sum().reshape(1)
+    if ep_idx:
+      total_ep = total_ep + parts.index_select(0, self._SlotIndex(ep_idx, parts.device)).sum().reshape(1)
     if any_ep:
       self._pre_ep_sumsq = total_ep
     if small:
@@ -861,7 +879,7 @@ class XLAShardingAdafactorOptimizer(torch.optim.Optimizer):
   """The same Adafactor as a plain `torch.optim.Optimizer` (ref :905, the raw optimizer the
   `XLAShardingAdafactor` layer wraps): for code that drives its own training loop.
   `learning_rate` / `decay_rate` may be numbers or zero-arg callables evaluated every step.
-  Runs the fused sm_100a kernels on CUDA parameters, the eager formulation elsewhere."""
+  Runs the fused sm_90a kernels on CUDA parameters, the eager formulation elsewhere."""
 
   def __init__(self, params, multiply_by_parameter_scale=True, learning_rate=None,
                decay_rate=None, beta1=0.0, clipping_threshold=1.0, factored=True,

@@ -2,7 +2,7 @@
 `preconditioner_op_kernels.cc`: `ComputePreconditioners` / `GetPreconditioners`).
 
 The reference ships gradient statistics to a pool of CPU sessions that run the inverse
-p-th-root graph while training continues with stale preconditioners. The B200 design keeps
+p-th-root graph while training continues with stale preconditioners. The H100 design keeps
 the statistics on the device and runs the coupled Newton iteration on a *low-priority CUDA
 stream*: training kernels on the main stream are never blocked, a finished solve is published
 when its event has fired, and readers get `(preconditioner, ok)` exactly like the reference

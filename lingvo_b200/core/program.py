@@ -7,7 +7,7 @@ Reference `lingvo/core/program.py`: `BaseProgram` (:75), `TrainProgram` (:441;
 (:2329), `MLPerfProgramSchedule`, `SimpleProgramScheduleForTask` (:2705),
 `UpdateProgramSchedule` (:2835).
 
-B200-first: a program is "run N steps of task X on this process group".
+H100-first: a program is "run N steps of task X on this process group".
 `TrainProgram.Run` executes `steps_per_loop` eager steps and syncs scalar
 metrics to the host **once per loop** (the TPU-loop analogue); eval/decode
 accumulate metrics on device (`DeviceEvalMetrics`).

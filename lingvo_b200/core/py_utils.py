@@ -10,7 +10,7 @@ helpers (:3084-3500), metric averaging (:3641-3689), variational noise
 AuxLossContext (:6572), trainable-var filters (:6610), BlockDiagonalMatmul
 (:6645), processed-checkpoint bookkeeping (:6759), Timer (:6890).
 
-Design differences (B200/PyTorch-first): variables are `torch.nn.Parameter`s
+Design differences (H100/PyTorch-first): variables are `torch.nn.Parameter`s
 created directly on the cluster's current device; gradients come from autograd
 (`torch.autograd.grad`), initializers are a method-name → function table, and
 thread-local *context stacks* are tiny `_Stack` objects.

@@ -12,7 +12,7 @@ Capability parity with reference `lingvo/core/quant_utils.py`:
   * `SymmetricScheduledClipQDomain` (:1530), `PassiveAsymQDomain` (:1606) with its counted
     min/max accumulator (:1582).
 
-B200 notes. Everything here is elementwise device work with *no host synchronisation*:
+H100 notes. Everything here is elementwise device work with *no host synchronisation*:
 ranges are 0-d device tensors (batch min/max, EMA state variables), the delayed-start and
 clip→quantize switches are `torch.where` on values derived from the global step, and the
 fake-quant op itself is a single fused expression with a straight-through gradient — so a

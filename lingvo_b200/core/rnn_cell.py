@@ -5,7 +5,7 @@ Cell contract (ref :37-211): `zero_state(theta, batch_size)` → state NestedMap
 `inputs = NestedMap(act=[tensor, …], padding=[B, 1])`; `GetOutput(state)`.
 Padded batch rows carry their previous state forward.
 
-B200 design: every cell splits its step into
+H100 design: every cell splits its step into
   * `ProjectInput(theta, acts [T, B, D])` — the input half of the gate GEMM,
     hoisted out of the time loop and run ONCE for the whole sequence on the
     tensor cores, and

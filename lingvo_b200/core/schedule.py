@@ -3,7 +3,7 @@
 Same catalogue and formulas as reference `lingvo/core/schedule.py` (:25-998):
 every schedule is a layer with `Value(step=None) -> float`.
 
-B200-first difference: the global step lives on the host, so a schedule value
+H100-first difference: the global step lives on the host, so a schedule value
 is a *python float* computed with `math` — no device op, no sync. The value is
 handed to the fused optimizer kernels as a scalar argument.
 """

@@ -18,7 +18,7 @@ class BlockSparseAttention(MultiHeadedSelfAttention):
   """Block-sparse attention with the diagonal band only (ref :30; BigBird, arXiv 2007.14062,
   without global / random blocks): query block l attends to key block l and nothing else.
 
-  B200 mapping: a block-diagonal attention *is* a batched dense attention — the `L = T / w`
+  H100 mapping: a block-diagonal attention *is* a batched dense attention — the `L = T / w`
   blocks are folded into the batch dimension (`[B, T, N, H] → [B·L, w, N, H]`, a free view),
   and the regular attention core (flash kernel on the device) runs on B·L short sequences.
   Cost O(T·w) instead of O(T²), and no `[B, N, L, w, w]` mask tensor is materialised: key

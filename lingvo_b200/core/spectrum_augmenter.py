@@ -18,7 +18,7 @@ reference:
     (counter-based hash evaluated on the device — no host round trip), which is what
     federated / replayable training needs (ref :145).
 
-B200 design. All randomness is drawn on the device (torch generator, or the stateless
+H100 design. All randomness is drawn on the device (torch generator, or the stateless
 hash), every mask is built by broadcast comparisons, and nothing synchronises with the host,
 so augmentation is a handful of elementwise kernels inside the captured train step. This
 base class keeps the reference's explicit `[B, N, N]` warp matrices (small batched GEMMs on

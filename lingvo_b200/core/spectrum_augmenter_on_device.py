@@ -2,7 +2,7 @@
 (ref `lingvo/core/spectrum_augmenter_on_device.py`).
 
 The reference's on-device variant rewrites the base layer's einsums into forms its target
-accelerator executes well. The B200 equivalent changes the *algorithms* that were shaped by
+accelerator executes well. The H100 equivalent changes the *algorithms* that were shaped by
 a matrix unit into memory-lean ones, keeping the sampled augmentation identical to
 `SpectrumAugmenter` for the same random stream:
 

@@ -2,7 +2,7 @@
 (ref `lingvo/core/tpu_embedding_layers{,_v1,_v2}.py`, `tpu_embedding_manager.py`).
 
 On TPU these tables live in the embedding hardware with dedicated
-SGD/Adagrad/Adam/FTRL optimizers fed by "send gradients" ops. The B200 equivalent:
+SGD/Adagrad/Adam/FTRL optimizers fed by "send gradients" ops. The H100 equivalent:
 tables are row-sharded across ranks (`index % world == rank`), lookups are an
 all-to-all of ids + rows over NVLink, and the table optimizer is applied **sparsely**
 (only to the rows touched in the step) right after backward, outside the dense

@@ -5,7 +5,7 @@ Reference `lingvo/executor.py`: `GetExecutorParams` (:67-153),
 schedule, export metrics, should-stop}), multi-task sampling,
 `HostDrivenExecutor` (:622).
 
-On B200 the executor is the SPMD entrypoint: every rank runs the same
+On H100 the executor is the SPMD entrypoint: every rank runs the same
 schedule; the train program's model is shared (by Parameter aliasing) with
 the eval/decode programs of the same rank, so no checkpoint round-trip is
 needed between train and eval.

@@ -19,7 +19,7 @@ Embedding → attention LSTM (input `[emb_t ; context_{t-1}]`, its output querie
     per-token or per-sequence averaging, `token_normalized_per_seq_loss`, several weighted
     logit heads (`logit_types`), per-sequence losses for MWER-style training.
 
-B200 notes. Two execution plans share the same cells and weights:
+H100 notes. Two execution plans share the same cells and weights:
   * the *sequence plan* (teacher forcing, no per-step feedback): the attention LSTM runs its
     step loop, but the upper LSTMs and the softmax run over the whole `[T, B, ·]` sequence —
     their input GEMMs are hoisted out of the time loop onto the tensor cores;

@@ -85,7 +85,7 @@ class WordLevelOneBwdsBase(base_model_params.SingleTaskModelParams):
 
 @model_registry.RegisterSingleTaskModel
 class WordLevelOneBwdsSimpleSampledSoftmax(WordLevelOneBwdsBase):
-  """Sampled-softmax variant (ref :134). On B200 the full 793k softmax fits the
+  """Sampled-softmax variant (ref :134). On H100 the full 793k softmax fits the
   fused chunked LM-head kernel, so `NUM_SAMPLED` only bounds its chunk size."""
 
   def Task(self):
@@ -109,7 +109,7 @@ class WordLevelOneBwdsSimpleSampledSoftmaxTiny(WordLevelOneBwdsSimpleSampledSoft
 
 @model_registry.RegisterSingleTaskModel
 class OneBwdsTransformerLm(WordLevelOneBwdsBase):
-  """Transformer LM on the same data (B200 flagship-style stack)."""
+  """Transformer LM on the same data (H100 flagship-style stack)."""
 
   VOCAB_SIZE = 32000
   MODEL_DIM = 1024

@@ -4,7 +4,7 @@ inference subgraph the reference exports for serving.
 
 `Inference()['default'](src_strings)` (ref `_InferenceSubgraph_Default` :37): tokenise the raw
 strings with the input generator's tokenizer (padded to `source_max_length`), encode, beam
-search, and convert the top-k hypotheses back to strings. On the B200 serving path the
+search, and convert the top-k hypotheses back to strings. On the H100 serving path the
 encoder/decoder math runs on the device; only tokenisation and detokenisation are host work.
 """
 

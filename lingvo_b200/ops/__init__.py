@@ -1,4 +1,4 @@
-"""Native (sm_100a CUDA / C++) ops of lingvo_b200.
+"""Native (sm_90a CUDA / C++) ops of lingvo_b200.
 
 `native()` returns the in-tree extension module `lingvo_b200/ops/_C.so`
 (built by `python -m lingvo_b200.ops.build`). On a GPU box a missing
@@ -62,7 +62,7 @@ def has_native() -> bool:
 
 
 def use_cuda_kernels(*tensors) -> bool:
-  """True when the fused sm_100a path must be taken for these tensors."""
+  """True when the fused sm_90a path must be taken for these tensors."""
   if not tensors or not all(t.is_cuda for t in tensors if t is not None):
     return False
   if os.environ.get('LINGVO_B200_DISABLE_KERNELS', '0') == '1':

@@ -120,7 +120,7 @@ class _RelBiasAttnFn(torch.autograd.Function):
 
   forward : `build_rel_bias` (ours) → cuDNN fused attention (library, like
             cuBLAS for plain GEMMs) producing O and the log-sum-exp.
-  backward: cuDNN fused backward for dQ/dK/dV + `rel_bias_grad` (our tcgen05
+  backward: cuDNN fused backward for dQ/dK/dV + `rel_bias_grad` (our wgmma
             kernel) for the bias-table gradient, which cuDNN cannot produce.
   """
 
@@ -182,7 +182,7 @@ def rel_bias_attention(q, k, v, rel, mask=None, scale=1.0, causal=False):
                               float(scale), bool(causal))
 
 
-# ------------------------------------------------------------ tcgen05 flash attention ----
+# ------------------------------------------------------------ wgmma flash attention ----
 def flash_attention_ref(q, k, v, rel=None, seg=None, pos=None, scale=1.0, causal=False):
   """fp32 oracle of `flash_attention`: packed-input mask built from segment ids / positions
   (visible ⇔ same non-zero segment and, if causal, pos_k <= pos_q) + Toeplitz bias."""
@@ -203,7 +203,7 @@ def flash_attention_ref(q, k, v, rel=None, seg=None, pos=None, scale=1.0, causal
 
 
 class _FlashAttnFn(torch.autograd.Function):
-  """Our tcgen05 flash attention (csrc/flash_attn.cu): forward, dQ/dK/dV and the gradient
+  """Our wgmma flash attention (csrc/flash_attn.cu): forward, dQ/dK/dV and the gradient
   of the relative-bias table in two kernels; no `[B,H,L,L]` tensor, no library call."""
 
   @staticmethod

@@ -1,7 +1,7 @@
 """In-tree build of the native extension `lingvo_b200/ops/_C.so`.
 
 `python -m lingvo_b200.ops.build` cross-compiles every `csrc/*.cu|*.cpp` for
-sm_100a (`-gencode arch=compute_100a,code=sm_100a -lineinfo`) with nvcc / g++
+sm_90a (`-gencode arch=compute_90a,code=sm_90a -lineinfo`) with nvcc / g++
 and links against the installed libtorch. Object files are cached under
 `csrc/_obj/` and rebuilt when the source (or any header) is newer. The `.so`
 stays in-tree so it travels with the repo snapshot to GPU boxes.
@@ -23,7 +23,7 @@ OBJ = os.path.join(CSRC, '_obj')
 TARGET = os.path.join(HERE, '_C.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 
-ARCH_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a']
 
 
 def _TorchPaths():

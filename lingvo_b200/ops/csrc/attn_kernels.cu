@@ -4,12 +4,12 @@
 //       one pass, never materialises the fp32 Toeplitz or the broadcast sum.
 //   rel_bias_grad  : d rel[h, i-j+L-1] = sum_b sum_{(i,j) on that diagonal} dS[b,h,i,j],
 //       dS = P o (dP - delta),  P = exp(scale*QK^T + bias - lse),  dP = dO V^T.
-//       tcgen05 kernel: both 128x128x128 GEMMs of a (h, i-block, j-block) tile are
-//       issued by one thread into TMEM (S and dP, double buffered over the batch
-//       loop), operands arrive by TMA (SWIZZLE_128B), the four epilogue warps
-//       recompute the softmax from the saved log-sum-exp, accumulate dS over the
-//       batch in registers and reduce it along diagonals in shared memory, so
-//       neither P, dS nor the [H,L,L] bias gradient ever reaches HBM.
+//       wgmma kernel: both 128x128x128 GEMMs of a (h, i-block, j-block) tile are
+//       computed by two warpgroups into registers, operands arrive by TMA
+//       (SWIZZLE_128B) through a three-slot ring, the warpgroups recompute the
+//       softmax from the saved log-sum-exp, accumulate dS over the batch in
+//       registers and reduce it along diagonals in shared memory, so neither P,
+//       dS nor the [H,L,L] bias gradient ever reaches HBM.
 //
 // Layouts: q,k,v,dO  [B, L, H, D] bf16 (BLHD, D = 128);  lse, delta [B, H, L] fp32;
 //          bias [B, H, L, L] bf16;  rel / drel [H, 2L-1] fp32.
@@ -91,8 +91,8 @@ constexpr int kChunkBytes = kT * 64 * 2;      // one [128 x 64] SW128 sub-tile =
 constexpr int kTileBytes = 2 * kChunkBytes;   // [128 x 128] operand = 32 KiB
 constexpr int kSlotBytes = 2 * kTileBytes;    // A + B operand of one GEMM = 64 KiB
 constexpr int kSlots = 3;
-constexpr int kThreads = 384;                 // 4 control warps + 8 epilogue warps
-constexpr uint32_t kTmemCols = 512;           // 2 stages x (S | dP) x 128 columns
+constexpr int kConsumers = 256;               // two warpgroups x 64 query rows
+constexpr int kThreads = kConsumers + 128;    // + the TMA producer warpgroup
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
@@ -110,6 +110,8 @@ struct GradParams {
   int causal;            // skip tiles strictly above the diagonal
 };
 
+// S = Q·K^T and dP = dO·V^T of one (i-block, j-block) tile per batch element, by wgmma into
+// registers: warpgroup g owns query rows [64g, 64g + 64) and accumulates dS over the batch.
 __global__ void __launch_bounds__(kThreads, 1)
 rel_bias_grad_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                      const __grid_constant__ CUtensorMap map_do, const __grid_constant__ CUtensorMap map_v,
@@ -126,45 +128,30 @@ rel_bias_grad_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kSlots * kSlotBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kSlots;
-  uint64_t* tmem_full_bar = bars + 2 * kSlots;
-  uint64_t* tmem_empty_bar = bars + 2 * kSlots + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * kSlots + 4);
-  float* sdiag = reinterpret_cast<float*>(bars + 2 * kSlots + 6);   // [256]
+  float* sdiag = reinterpret_cast<float*>(bars + 2 * kSlots + 2);   // [256]
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int i0 = i_blk * kT, j0 = j_blk * kT;
 
-  if (warp_idx == 0 && lane == 0) {
+  if (threadIdx.x == kConsumers) {
     tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_k);
     tma_prefetch_desc(&map_do);
     tma_prefetch_desc(&map_v);
-  }
-  if (warp_idx == 1 && lane == 0) {
     for (int s = 0; s < kSlots; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&tmem_full_bar[s]), 1);
-      mbar_init(smem_u32(&tmem_empty_bar[s]), 8);
+      mbar_init(smem_u32(&empty_bar[s]), kConsumers / 32);
     }
     fence_barrier_init();
   }
-  if (warp_idx == 2) {
-    tmem_alloc<kTmemCols>(smem_u32(tmem_ptr_smem));
-    tmem_relinquish();
-  }
   if (threadIdx.x < 256) sdiag[threadIdx.x] = 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp_idx == 0) {
+  if (warp_idx >= kConsumers / 32) {
     // ============================ TMA producer ============================
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == kConsumers) {
       int slot = 0;
       uint32_t phase = 0;
       for (int b = 0; b < p.B; ++b) {
@@ -185,111 +172,82 @@ rel_bias_grad_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
         }
       }
     }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    // ============================= MMA issuer =============================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(1, 1, false, false, kT, kT);
-      int slot = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int b = 0; b < p.B; ++b) {
-        mbar_wait(smem_u32(&tmem_empty_bar[acc]), acc_phase ^ 1);
-        tc_fence_after();
-        for (int g = 0; g < 2; ++g) {
-          mbar_wait(smem_u32(&full_bar[slot]), phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + slot * kSlotBytes);
-          const uint32_t sb = sa + kTileBytes;
-          const uint32_t tmem_d = tmem_base + acc * 256 + g * 128;
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const uint64_t adesc = make_smem_desc_sw128(sa + c * kChunkBytes + j * 32, 16, 1024);
-              const uint64_t bdesc = make_smem_desc_sw128(sb + c * kChunkBytes + j * 32, 16, 1024);
-              umma_f16(tmem_d, adesc, bdesc, idesc, (c | j) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(smem_u32(&empty_bar[slot]));
-          if (++slot == kSlots) { slot = 0; phase ^= 1; }
-        }
-        umma_commit(smem_u32(&tmem_full_bar[acc]));
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-    __syncwarp();
-  } else if (warp_idx >= 4) {
-    // ======================= softmax-recompute epilogue ====================
-    // 8 warps: warp w reads TMEM lanes 32·(w % 4).. (one query row per lane) and owns one
-    // half of the tile's 128 key columns, so every SM sub-partition has two epilogue warps
-    // to switch between (with four warps each scheduler had a single warp and every
-    // FFMA / MUFU latency was exposed) and the per-thread tile is 64 registers, not 128.
-    const int q = warp_idx & 3;
-    const int half = (warp_idx - 4) >> 2;
-    const int row = q * 32 + lane;
-    const int i = i0 + row;
-    constexpr int kCols = kT / 2;
-    constexpr float kLog2e = 1.4426950408889634f;
-    const float sl2 = p.scale * kLog2e;
-    float ds[kCols];
-#pragma unroll
-    for (int c = 0; c < kCols; ++c) ds[c] = 0.f;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int b = 0; b < p.B; ++b) {
-      const long long bh = static_cast<long long>(b) * p.H + h;
-      const float lse2 = p.lse[bh * p.L + i] * kLog2e;
-      const float delta = p.delta[bh * p.L + i];
-      const __nv_bfloat16* brow = p.bias + (bh * p.L + i) * p.L + j0 + half * kCols;
-      mbar_wait(smem_u32(&tmem_full_bar[acc]), acc_phase);
-      tc_fence_after();
-      const uint32_t t_s = tmem_base + acc * 256 + half * kCols + (static_cast<uint32_t>(q * 32) << 16);
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t vs[32], vp[32];
-        tmem_ld_32x32b_x32(t_s + c * 32, vs);
-        tmem_ld_32x32b_x32(t_s + 128 + c * 32, vp);
-        int4 bv[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) bv[u] = ld_nc_v4(brow + c * 32 + u * 8);
-        tmem_ld_wait();
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const uint32_t w[4] = {static_cast<uint32_t>(bv[u].x), static_cast<uint32_t>(bv[u].y),
-                                 static_cast<uint32_t>(bv[u].z), static_cast<uint32_t>(bv[u].w)};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float2 bb = unpack_bf16x2(w[e]);
-            const int k0 = u * 8 + e * 2;
-            // p = exp(s·scale + bias − lse) = 2^(s·scale·log2e + (bias·log2e − lse·log2e))
-            const float p0 = fast_exp2(fmaf(__uint_as_float(vs[k0]), sl2, fmaf(bb.x, kLog2e, -lse2)));
-            const float p1 = fast_exp2(fmaf(__uint_as_float(vs[k0 + 1]), sl2, fmaf(bb.y, kLog2e, -lse2)));
-            ds[c * 32 + k0] = fmaf(p0, __uint_as_float(vp[k0]) - delta, ds[c * 32 + k0]);
-            ds[c * 32 + k0 + 1] = fmaf(p1, __uint_as_float(vp[k0 + 1]) - delta, ds[c * 32 + k0 + 1]);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&tmem_empty_bar[acc]));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-    // Diagonal (Toeplitz) reduction: element (row, col) lies on diagonal row - col.
-#pragma unroll
-    for (int c = 0; c < kCols; ++c) atomicAdd(&sdiag[row - (half * kCols + c) + (kT - 1)], ds[c]);
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    float* out = p.drel + static_cast<long long>(h) * (2 * p.L - 1) + (i0 - j0) + (p.L - 1) - (kT - 1);
-    for (int t = half * kT + row; t < 2 * kT - 1; t += 2 * kT) atomicAdd(out + t, sdiag[t]);
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc<kTmemCols>(tmem_base);
+  // ======================= softmax-recompute warpgroups ====================
+  setmaxnreg_inc<232>();
+  const int wg = warp_idx >> 2;
+  const int row0 = wg * 64 + (warp_idx & 3) * 16 + (lane >> 2);   // tile rows row0, row0 + 8
+  const int cq = (lane & 3) * 2;
+  constexpr float kLog2e = 1.4426950408889634f;
+  const float sl2 = p.scale * kLog2e;
+  float ds[64];
+#pragma unroll
+  for (int c = 0; c < 64; ++c) ds[c] = 0.f;
+  int slot = 0;
+  uint32_t phase = 0;
+  for (int b = 0; b < p.B; ++b) {
+    const long long bh = static_cast<long long>(b) * p.H + h;
+    float sacc[64], pacc[64];
+#pragma unroll
+    for (int c = 0; c < 64; ++c) { sacc[c] = 0.f; pacc[c] = 0.f; }
+    int slots[2];
+#pragma unroll
+    for (int g = 0; g < 2; ++g) {
+      slots[g] = slot;
+      mbar_wait(smem_u32(&full_bar[slot]), phase);
+      const uint32_t sa = smem_u32(smem + slot * kSlotBytes);
+      const uint32_t sb = sa + kTileBytes;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const uint64_t adesc =
+            make_smem_desc_sw128(sa + (kk >> 2) * kChunkBytes + wg * 8192 + (kk & 3) * 32, 16, 1024);
+        const uint64_t bdesc = make_smem_desc_sw128(sb + (kk >> 2) * kChunkBytes + (kk & 3) * 32, 16, 1024);
+        if (g == 0) wgmma_m64n128k16<0, 0>(sacc, adesc, bdesc, 1);
+        else wgmma_m64n128k16<0, 0>(pacc, adesc, bdesc, 1);
+      }
+      wgmma_commit();
+      if (++slot == kSlots) { slot = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(sacc);
+    wgmma_fence_regs(pacc);
+    __syncwarp();
+    if (lane == 0) {
+      mbar_arrive(smem_u32(&empty_bar[slots[0]]));
+      mbar_arrive(smem_u32(&empty_bar[slots[1]]));
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int qi = i0 + row0 + 8 * i;
+      const float lse2 = p.lse[bh * p.L + qi] * kLog2e;
+      const float delta = p.delta[bh * p.L + qi];
+      const __nv_bfloat16* brow = p.bias + (bh * p.L + qi) * p.L + j0 + cq;
+#pragma unroll
+      for (int n = 0; n < 16; ++n) {
+        const float2 bb = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(brow + n * 8));
+        const int e = 4 * n + 2 * i;
+        // p = exp(s·scale + bias − lse) = 2^(s·scale·log2e + (bias·log2e − lse·log2e))
+        const float p0 = fast_exp2(fmaf(sacc[e], sl2, fmaf(bb.x, kLog2e, -lse2)));
+        const float p1 = fast_exp2(fmaf(sacc[e + 1], sl2, fmaf(bb.y, kLog2e, -lse2)));
+        ds[e] = fmaf(p0, pacc[e] - delta, ds[e]);
+        ds[e + 1] = fmaf(p1, pacc[e + 1] - delta, ds[e + 1]);
+      }
+    }
   }
+  // Diagonal (Toeplitz) reduction: element (row, col) lies on diagonal row - col.
+#pragma unroll
+  for (int n = 0; n < 16; ++n)
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        atomicAdd(&sdiag[row0 + 8 * i - (n * 8 + cq + j) + (kT - 1)], ds[4 * n + 2 * i + j]);
+  named_bar_sync(1, kConsumers);
+  float* out = p.drel + static_cast<long long>(h) * (2 * p.L - 1) + (i0 - j0) + (p.L - 1) - (kT - 1);
+  if (threadIdx.x < 2 * kT - 1) atomicAdd(out + threadIdx.x, sdiag[threadIdx.x]);
 }
 
 }  // namespace

@@ -15,7 +15,7 @@ void RegisterAll(pybind11::module& m);
 }  // namespace lb
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "lingvo_b200 sm_100a kernels";
+  m.doc() = "lingvo_b200 sm_90a kernels";
   m.def("gemm_bf16", &lb::gemm_bf16, py::arg("a"), py::arg("b"), py::arg("a_kmajor") = true,
         py::arg("b_kmajor") = true, py::arg("bias") = py::none(), py::arg("act") = 0,
         py::arg("aux") = py::none(), py::arg("aux_mode") = 0, py::arg("row_scale") = py::none(),

@@ -185,8 +185,9 @@ int Blocks(long long n8) {
 }  // namespace
 
 // `max_blocks` > 0 caps the grid: a bucket reduced on the communication stream *during*
-// backward only needs enough CTAs to keep NVLink busy (≈2 µs × 900 GB/s of 16-byte loads in
-// flight ≈ 32–64 CTAs) and must leave the SMs to the GEMMs it overlaps with.
+// backward only needs enough CTAs to keep NVLink busy (≈2 µs of latency × 450 GB/s per
+// direction on NVLink-4 ≈ 0.9 MB of 16-byte loads in flight ≈ 16–32 CTAs) and must leave the
+// SMs to the GEMMs it overlaps with.
 void allreduce_mean_bf16(const torch::Tensor& peer_ptrs_cpu, int64_t shard_elems, int64_t rank,
                          int64_t world, double scale, int64_t device, bool store_all,
                          const c10::optional<torch::Tensor>& sumsq, int64_t max_blocks) {

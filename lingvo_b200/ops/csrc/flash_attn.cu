@@ -1,4 +1,4 @@
-// tcgen05 flash attention with a learned Toeplitz (T5) relative-position bias
+// Hopper (sm_90a) flash attention with a learned Toeplitz (T5) relative-position bias
 // (SURVEY K7/K8; reference semantics `gshard_builder.py:2697-2804,1431-1514`).
 //
 //   O[b,i,h,:] = softmax_j( scale·q_i·k_j + rel[h, i-j+L-1] + mask(b,i,j) ) · v_j
@@ -9,24 +9,14 @@
 // reach HBM; the gradient of the bias table is folded into the backward kernel.
 //
 // Both kernels use the same recipe: operand tiles [128 x 128] bf16 arrive by TMA as two
-// [128 rows x 64 cols] SWIZZLE_128B chunks; one elected thread issues tcgen05.mma
-// (128x128x16, fp32 accumulators in TMEM); eight epilogue warps (one query row per TMEM
-// lane, two column halves) do the softmax math between the GEMMs. The same physical smem
-// layout serves as a K-major operand (rows = M/N index) or an MN-major operand (rows = K
-// index) by changing only the descriptor, so no transposes are ever materialised.
-//
-//   forward  (CTA = (i-block, h, b)):  loop over key blocks:
-//       S = Q·K^T -> TMEM | online softmax, P (bf16) -> smem | PV = P·V -> TMEM |
-//       O = alpha·O + PV in registers.  K/V double-buffered; S(j+1) is issued right
-//       behind PV(j) so the tensor pipe works while the warps rescale O.
-//   backward (CTA = (j-block, h, b)):  loop over query blocks (FlashAttention-2 order):
-//       S = Q·K^T, dP = dO·V^T | P = exp2(S - lse), dS = P∘(dP - delta) |
-//       dV += P^T·dO | dK += dS^T·Q | dQ_tile = dS·K -> fp32 red.add into dq_acc;
-//       d rel[h, i-j+L-1] += Σ dS along diagonals (warp-shuffle skew, no smem atomics).
-//       dK, dV stay in TMEM for the whole loop (S | dP | dV | dK = 512 columns).
+// [128 rows x 64 cols] SWIZZLE_128B chunks into a shared-memory ring fed by one producer
+// thread; two consumer warpgroups issue wgmma (fp32 accumulators in registers) and do the
+// softmax math between the GEMMs. The same physical smem layout serves as a K-major
+// operand (rows = M/N index) or an MN-major operand (rows = K index) by changing only the
+// descriptor and the wgmma transpose bit, so no transposes are ever materialised.
 //
 // Layouts: q,k,v,dO [B, L, H, D=128] bf16 views (strides (*, *, D, 1));  O, dK, dV
-// [B, L, H, D] contiguous bf16;  dq_acc [B, L, H, D] fp32;  lse, delta [B, H, L] fp32;
+// [B, L, H, D] contiguous bf16;  dq_part [Jc, B, L, H, D] fp32;  lse, delta [B, H, L] fp32;
 // rel / drel [H, 2L-1] fp32;  segment ids / positions [B, L] int32 (optional).
 
 #include <ATen/cuda/CUDAContext.h>
@@ -50,7 +40,8 @@ constexpr int kT = 128;                      // tile edge (queries / keys)
 constexpr int kD = 128;                      // head dim
 constexpr int kChunk = kT * 64 * 2;          // [128 x 64] SW128 chunk = 16 KiB
 constexpr int kTile = 2 * kChunk;            // [128 x 128] bf16 operand = 32 KiB
-constexpr int kThreads = 320;                // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
+constexpr int kConsumers = 256;              // two warpgroups (warps 0..7)
+constexpr int kThreads = kConsumers + 128;   // + the TMA producer warpgroup (warps 8..11)
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 constexpr float kMasked = -1.0e9f;           // additive mask value (log2 domain, finite)
@@ -65,17 +56,6 @@ __device__ __forceinline__ float lg2(float x) {
   asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c,
-                                             uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c),
-               "r"(d)
-               : "memory");
-}
-__device__ __forceinline__ void red_add_v4_f32(float* p, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c),
-               "f"(d)
-               : "memory");
-}
 // Explicit shared-space accesses: the tile base is re-aligned through integer arithmetic,
 // after which the compiler can only emit *generic* LD/ST for C++ pointers into it.
 __device__ __forceinline__ float lds_f32(uint32_t a) {
@@ -88,47 +68,25 @@ __device__ __forceinline__ int lds_s32(uint32_t a) {
   asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(a));
   return v;
 }
-__device__ __forceinline__ int lds_s16(uint32_t a) {
-  int v;
-  asm volatile("ld.shared.s16 %0, [%1];" : "=r"(v) : "r"(a));
-  return v;
-}
 __device__ __forceinline__ void sts_f32(uint32_t a, float v) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory");
 }
 __device__ __forceinline__ void sts_s32(uint32_t a, int v) {
   asm volatile("st.shared.s32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
 }
-__device__ __forceinline__ void sts_s16(uint32_t a, int v) {
-  asm volatile("st.shared.s16 [%0], %1;" ::"r"(a), "r"(v) : "memory");
-}
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// smem byte offset of the 16-byte unit holding columns [8u, 8u+8) of row r in a
-// [128 x 128] tile stored as two SW128 chunks of 64 columns.
-__device__ __forceinline__ uint32_t tile_unit_off(int r, int col8) {
-  const int chunk = col8 >> 3;               // 64 columns = 8 units per chunk
-  const int u = col8 & 7;
-  return static_cast<uint32_t>(chunk * kChunk + r * 128 + ((u ^ (r & 7)) << 4));
+// Byte offset of the bf16 pair (col, col + 1) of row r in a SW128 operand whose rows hold 64
+// columns (128 B); 64-column chunks of `chunk_bytes` each (col < 64 for a single chunk).
+__device__ __forceinline__ uint32_t sw128_off(int r, int col, uint32_t chunk_bytes) {
+  const int c = col & 63;
+  return static_cast<uint32_t>(col >> 6) * chunk_bytes +
+         static_cast<uint32_t>(r * 128 + (((c >> 3) ^ (r & 7)) << 4) + (c & 7) * 2);
 }
-
-// Issue one 128x128x128 GEMM as 8 UMMAs. kAMn / kBMn: operand is MN-major (rows = K index).
-template <bool kAMn, bool kBMn>
-__device__ __forceinline__ void issue_gemm(uint32_t tmem_d, uint32_t sa, uint32_t sb,
-                                           bool accumulate) {
-  constexpr uint32_t idesc = make_idesc(1, 1, kAMn, kBMn, kT, kT);
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    // K-major: 64-wide K chunks are kChunk apart, 16-element steps are 32 B inside the
-    //          128 B swizzle row.  MN-major: 16 K-rows of 128 B per step; the two 64-wide
-    //          MN chunks are kChunk apart (LBO), 8-row groups 1 KiB (SBO).
-    const uint64_t adesc = kAMn ? make_smem_desc_sw128(sa + k * (16 * 128), kChunk, 1024)
-                                : make_smem_desc_sw128(sa + (k >> 2) * kChunk + (k & 3) * 32, 16, 1024);
-    const uint64_t bdesc = kBMn ? make_smem_desc_sw128(sb + k * (16 * 128), kChunk, 1024)
-                                : make_smem_desc_sw128(sb + (k >> 2) * kChunk + (k & 3) * 32, 16, 1024);
-    umma_f16(tmem_d, adesc, bdesc, idesc, (accumulate || k != 0) ? 1u : 0u);
-  }
+__device__ __forceinline__ void sts_b32(uint32_t a, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
 }
+__device__ __forceinline__ uint64_t kdesc(uint32_t a) { return make_smem_desc_sw128(a, 16, 1024); }
+__device__ __forceinline__ uint64_t mndesc(uint32_t a) { return make_smem_desc_sw128(a, kChunk, 1024); }
 
 __device__ __forceinline__ void load_tile(uint32_t dst, const CUtensorMap* map, uint32_t bar,
                                           int h, int row0, int b) {
@@ -172,16 +130,12 @@ struct FwdParams {
   float scale;
 };
 
-// smem: Q | K x2 | V | P x2 (each 32 KiB) + 8 KiB of barriers / per-block tables.
-constexpr size_t kFwdSmem = kTile * 6 + 8192 + 1024;
+// smem: Q | (K, V) x 2 stages | P x 2 warpgroups (16 KiB each) + barriers / per-block tables.
+constexpr size_t kFwdSmem = kTile * 6 + 4096 + 1024;
 
-// Software pipeline (steady state, block j):
-//   tensor pipe : ... PV(j-1) | S(j+1) ...          (issued while the warps work on block j)
-//   warps       : softmax(j) -> P(j) to smem -> signal -> O = alpha·O + PV(j-1)
-// S and PV are double-buffered in TMEM (4 x 128 columns), P in smem, K has two stages and
-// V one (V(j+1) is only needed after softmax(j+1)); the per-block bias/mask tables for
-// block j+1 are fetched while block j is processed. The warps never wait for a GEMM that
-// was not issued a whole softmax earlier.
+// K/V blocks stream through a two-stage TMA ring while each warpgroup runs
+//   S = Q·K^T (wgmma, registers) | online softmax | P (bf16) -> smem | O += P·V (wgmma)
+// on its 64 query rows.
 __global__ void __launch_bounds__(kThreads, 1)
 flash_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                  const __grid_constant__ CUtensorMap map_v, const FwdParams p) {
@@ -195,265 +149,184 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   const uint32_t s_q = smem_u32(smem);
-  const uint32_t s_k = s_q + kTile;                          // 2 stages
-  const uint32_t s_v = s_k + 2 * kTile;                      // 1 stage
-  const uint32_t s_p = s_v + kTile;                          // 2 buffers
+  const uint32_t s_kv = s_q + kTile;                         // stage s: K at +2s·kTile, V behind it
+  const uint32_t s_p = s_kv + 4 * kTile;                     // warpgroup g: +g·kTile/2
   uint8_t* meta = smem + kTile * 6;
   uint64_t* bars = reinterpret_cast<uint64_t*>(meta);
   uint64_t* q_bar = bars;                 // 1
-  uint64_t* k_full = bars + 1;            // 2
-  uint64_t* k_empty = bars + 3;           // 2
-  uint64_t* v_full = bars + 5;            // 1
-  uint64_t* v_empty = bars + 6;           // 1
-  uint64_t* s_full = bars + 7;            // 2
-  uint64_t* p_ready = bars + 9;           // 2
-  uint64_t* pv_full = bars + 11;          // 2
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 13);
-  const uint32_t s_xch = smem_u32(meta + 128);              // float [2][128]
-  const uint32_t s_tab = s_xch + 1024;                      // 2 x {rel[256] f32, seg[128], pos[128]}
-  constexpr int kTableBytes = 1024 + 512 + 512;
+  uint64_t* kv_full = bars + 1;           // 2
+  uint64_t* kv_empty = bars + 3;          // 2
+  const uint32_t s_rel = smem_u32(meta + 128);              // float [256]
+  const uint32_t s_seg = s_rel + 1024;                      // int [128]
+  const uint32_t s_pos = s_seg + 512;                       // int [128]
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp_idx == 0 && lane == 0) {
+  if (threadIdx.x == kConsumers) {
     tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_k);
     tma_prefetch_desc(&map_v);
     mbar_init(smem_u32(q_bar), 1);
     for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&k_full[s]), 1);
-      mbar_init(smem_u32(&k_empty[s]), 1);
-      mbar_init(smem_u32(&s_full[s]), 1);
-      mbar_init(smem_u32(&p_ready[s]), 8);
-      mbar_init(smem_u32(&pv_full[s]), 1);
+      mbar_init(smem_u32(&kv_full[s]), 1);
+      mbar_init(smem_u32(&kv_empty[s]), kConsumers / 32);
     }
-    mbar_init(smem_u32(v_full), 1);
-    mbar_init(smem_u32(v_empty), 1);
     fence_barrier_init();
   }
-  if (warp_idx == 1) {
-    tmem_alloc<512>(smem_u32(tmem_ptr_smem));
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  // S buffers: columns [0,128), [128,256);  PV buffers: [256,384), [384,512)
 
-  // ordered list of visible key blocks is implicit: every role walks jb = 0..nblk-1 and
-  // skips with the same predicate.
-  int n_vis = 0;
-  for (int jb = 0; jb < nblk; ++jb)
-    n_vis += pair_visible(p.mask, qmeta, block_meta(p.mask, b, nblk, jb)) ? 1 : 0;
-
-  if (warp_idx == 0) {
+  if (warp_idx >= kConsumers / 32) {
     // ============================ TMA producer ============================
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == kConsumers) {
       mbar_arrive_expect_tx(smem_u32(q_bar), kTile);
       load_tile(s_q, &map_q, smem_u32(q_bar), h, i0, b);
-      // K runs one block ahead of V: K(0), then for each visible block it: K(it+1), V(it).
-      int jk = 0;                                  // scan position of the K stream
-      int itk = 0;
-      auto next_k = [&]() {
-        while (jk < nblk && !pair_visible(p.mask, qmeta, block_meta(p.mask, b, nblk, jk))) ++jk;
-        if (jk >= nblk) return;
-        const int s = itk & 1;
-        mbar_wait(smem_u32(&k_empty[s]), ((itk >> 1) & 1) ^ 1);
-        const uint32_t fb = smem_u32(&k_full[s]);
-        mbar_arrive_expect_tx(fb, kTile);
-        load_tile(s_k + s * kTile, &map_k, fb, h, jk * kT, b);
-        ++itk;
-        ++jk;
-      };
-      next_k();
       int it = 0;
       for (int jb = 0; jb < nblk; ++jb) {
         if (!pair_visible(p.mask, qmeta, block_meta(p.mask, b, nblk, jb))) continue;
-        next_k();
-        mbar_wait(smem_u32(v_empty), (it & 1) ^ 1);
-        mbar_arrive_expect_tx(smem_u32(v_full), kTile);
-        load_tile(s_v, &map_v, smem_u32(v_full), h, jb * kT, b);
+        const int s = it & 1;
+        mbar_wait(smem_u32(&kv_empty[s]), ((it >> 1) & 1) ^ 1);
+        const uint32_t fb = smem_u32(&kv_full[s]);
+        mbar_arrive_expect_tx(fb, 2 * kTile);
+        load_tile(s_kv + 2 * s * kTile, &map_k, fb, h, jb * kT, b);
+        load_tile(s_kv + (2 * s + 1) * kTile, &map_v, fb, h, jb * kT, b);
         ++it;
       }
     }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    // ============================= MMA issuer =============================
-    if (lane == 0) {
-      mbar_wait(smem_u32(q_bar), 0);        // always: the Q load must land before the CTA exits
-      auto issue_s = [&](int it) {          // S(it) into S buffer it & 1 from K stage it & 1
-        const int s = it & 1;
-        mbar_wait(smem_u32(&k_full[s]), (it >> 1) & 1);
-        tc_fence_after();
-        issue_gemm<false, false>(tmem_base + s * 128, s_q, s_k + s * kTile, false);
-        umma_commit(smem_u32(&s_full[s]));
-        umma_commit(smem_u32(&k_empty[s]));
-      };
-      if (n_vis > 0) issue_s(0);
-      if (n_vis > 1) issue_s(1);
-      for (int it = 0; it < n_vis; ++it) {
-        const int s = it & 1;
-        mbar_wait(smem_u32(&p_ready[s]), (it >> 1) & 1);
-        mbar_wait(smem_u32(v_full), it & 1);
-        tc_fence_after();
-        issue_gemm<false, true>(tmem_base + 256 + s * 128, s_p + s * kTile, s_v, false);   // P·V
-        umma_commit(smem_u32(&pv_full[s]));
-        umma_commit(smem_u32(v_empty));
-        if (it + 2 < n_vis) issue_s(it + 2);      // S buffer `s` was drained before p_ready(it)
-      }
-    }
-    __syncwarp();
-  } else {
-    // ================= softmax / rescale warps (8 x 32 threads) =================
-    const int q4 = warp_idx & 3;                       // TMEM lane quarter of this warp
-    const int hf = (warp_idx - 2) >> 2;                // column half
-    const int r = q4 * 32 + lane;                      // query row inside the tile
-    const int et = (hf * 4 + ((q4 + 2) & 3)) * 32 + lane;   // 0..255, dense id for loads
-    const int i = i0 + r;
-    const long long bl = static_cast<long long>(b) * p.L;
-    const int segq = p.mask.seg ? p.mask.seg[bl + i] : 1;
-    const int posq = p.mask.pos ? p.mask.pos[bl + i] : i;
-    const float sl2 = p.scale * kLog2e;
-    const uint32_t lane_off = static_cast<uint32_t>(q4 * 32) << 16;
-    float o[64];
-#pragma unroll
-    for (int c = 0; c < 64; ++c) o[c] = 0.f;
-    float m_run = -INFINITY, l_run = 0.f;
-
-    // per-block tables → smem buffer `buf` (published by the next epi_bar_sync)
-    auto fetch_tables = [&](int jb, int buf) {
-      const uint32_t tb = s_tab + buf * kTableBytes;
-      const int j0 = jb * kT;
-      if (et < 255)
-        sts_f32(tb + et * 4,
-                p.rel ? p.rel[static_cast<long long>(h) * (2 * p.L - 1) + (i0 - j0 + p.L - 1) - 127 + et] * kLog2e
-                      : 0.f);
-      if (et < 128) {
-        sts_s32(tb + 1024 + et * 4, p.mask.seg ? p.mask.seg[bl + j0 + et] : 1);
-        sts_s32(tb + 1536 + et * 4, p.mask.pos ? p.mask.pos[bl + j0 + et] : j0 + et);
-      }
-    };
-    auto next_vis = [&](int jb) {
-      while (jb < nblk && !pair_visible(p.mask, qmeta, block_meta(p.mask, b, nblk, jb))) ++jb;
-      return jb;
-    };
-    // O = alpha·O + PV(buffer)
-    auto o_update = [&](int it, float alpha) {
-      const int s = it & 1;
-      mbar_wait(smem_u32(&pv_full[s]), (it >> 1) & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + 256 + s * 128 + lane_off + hf * 64 + cc * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int k = 0; k < 32; ++k)
-          o[cc * 32 + k] = fmaf(o[cc * 32 + k], alpha, __uint_as_float(v[k]));
-      }
-      tc_fence_before();
-    };
-
-    int jb = next_vis(0);
-    if (jb < nblk) fetch_tables(jb, 0);
-    float alpha_prev = 0.f;
-    for (int it = 0; it < n_vis; ++it) {
-      const int s = it & 1;
-      const uint32_t rel_a = s_tab + s * kTableBytes + (r + 127) * 4;   // rel_s[r - c + 127]
-      const uint32_t seg_a = s_tab + s * kTableBytes + 1024;
-      const uint32_t pos_a = seg_a + 512;
-      const bool full = pair_full(p.mask, qmeta, block_meta(p.mask, b, nblk, jb));
-      const int jb_next = next_vis(jb + 1);
-      epi_bar_sync();                                  // tables of block `it` are in place
-      if (jb_next < nblk) fetch_tables(jb_next, s ^ 1);    // buffer s^1: readers left it at the barrier
-      mbar_wait(smem_u32(&s_full[s]), (it >> 1) & 1);
-      tc_fence_after();
-      float sv[64];
-      float mloc = -INFINITY;
-#pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + s * 128 + lane_off + hf * 64 + cc * 32, v);
-        tmem_ld_wait();
-        if (full) {                    // interior block: bias only, no mask arithmetic
-#pragma unroll
-          for (int k = 0; k < 32; ++k) {
-            const int c = hf * 64 + cc * 32 + k;
-            const float x = fmaf(__uint_as_float(v[k]), sl2, lds_f32(rel_a - c * 4));
-            sv[cc * 32 + k] = x;
-            mloc = fmaxf(mloc, x);
-          }
-        } else {
-#pragma unroll
-          for (int k = 0; k < 32; ++k) {
-            const int c = hf * 64 + cc * 32 + k;
-            float x = fmaf(__uint_as_float(v[k]), sl2, lds_f32(rel_a - c * 4));
-            const bool vis = (segq == lds_s32(seg_a + c * 4)) && (segq != 0) &&
-                             (!p.mask.causal || posq >= lds_s32(pos_a + c * 4));
-            x = vis ? x : kMasked;
-            sv[cc * 32 + k] = x;
-            mloc = fmaxf(mloc, x);
-          }
-        }
-      }
-      sts_f32(s_xch + (hf * 128 + r) * 4, mloc);
-      epi_bar_sync();
-      const float m_new = fmaxf(m_run, fmaxf(mloc, lds_f32(s_xch + ((1 - hf) * 128 + r) * 4)));
-      const float alpha = ex2(m_run - m_new);
-      float lsum = 0.f;
-      const uint32_t s_pb = s_p + s * kTile;
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        uint32_t w[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float p0 = ex2(sv[u * 8 + 2 * e] - m_new);
-          const float p1 = ex2(sv[u * 8 + 2 * e + 1] - m_new);
-          lsum += p0 + p1;
-          w[e] = pack_bf16x2(p0, p1);
-        }
-        st_shared_v4(s_pb + tile_unit_off(r, hf * 8 + u), w[0], w[1], w[2], w[3]);
-      }
-      l_run = l_run * alpha + lsum;
-      m_run = m_new;
-      fence_proxy_async();          // P (generic-proxy stores) → visible to the MMA's async proxy
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&p_ready[s]));
-      // the previous block's P·V has been running during this softmax: fold it in now
-      if (it > 0) o_update(it - 1, alpha_prev);
-      alpha_prev = alpha;
-      jb = jb_next;
-    }
-    if (n_vis > 0) o_update(n_vis - 1, alpha_prev);
-    // ---- finalize: O / l, log-sum-exp ----
-    epi_bar_sync();
-    sts_f32(s_xch + (hf * 128 + r) * 4, l_run);
-    epi_bar_sync();
-    const float l_tot = l_run + lds_f32(s_xch + ((1 - hf) * 128 + r) * 4);
-    const float inv = l_tot > 0.f ? 1.f / l_tot : 0.f;      // query block that sees nothing: 0
-    __nv_bfloat16* dst = p.out + ((bl + i) * p.H + h) * kD + hf * 64;
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      int4 w;
-      w.x = pack_bf16x2(o[u * 8 + 0] * inv, o[u * 8 + 1] * inv);
-      w.y = pack_bf16x2(o[u * 8 + 2] * inv, o[u * 8 + 3] * inv);
-      w.z = pack_bf16x2(o[u * 8 + 4] * inv, o[u * 8 + 5] * inv);
-      w.w = pack_bf16x2(o[u * 8 + 6] * inv, o[u * 8 + 7] * inv);
-      st_v4(dst + u * 8, w);
-    }
-    if (hf == 0)
-      p.lse[(static_cast<long long>(b) * p.H + h) * p.L + i] =
-          l_tot > 0.f ? (m_run + lg2(l_tot)) * kLn2 : 0.f;
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+  // ================= softmax warpgroups (2 x 128 threads) =================
+  setmaxnreg_inc<232>();
+  const int wg = warp_idx >> 2;
+  const int pr0 = (warp_idx & 3) * 16 + (lane >> 2);       // rows pr0, pr0 + 8 of this warpgroup
+  const int cq = (lane & 3) * 2;
+  const long long bl = static_cast<long long>(b) * p.L;
+  const float sl2 = p.scale * kLog2e;
+  const uint32_t s_pw = s_p + wg * (kTile / 2);            // this warpgroup's P: [64 x 128]
+  int segq[2], posq[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int qi = i0 + wg * 64 + pr0 + 8 * i;
+    segq[i] = p.mask.seg ? p.mask.seg[bl + qi] : 1;
+    posq[i] = p.mask.pos ? p.mask.pos[bl + qi] : qi;
+  }
+  float o[64];
+#pragma unroll
+  for (int c = 0; c < 64; ++c) o[c] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  mbar_wait(smem_u32(q_bar), 0);
+
+  int it = 0;
+  for (int jb = 0; jb < nblk; ++jb) {
+    const int4 kmeta = block_meta(p.mask, b, nblk, jb);
+    if (!pair_visible(p.mask, qmeta, kmeta)) continue;
+    const int s = it & 1;
+    const int j0 = jb * kT;
+    const bool full = pair_full(p.mask, qmeta, kmeta);
+    named_bar_sync(1, kConsumers);                 // the previous block's tables are free
+    {
+      const int t = threadIdx.x;
+      if (t < 255)
+        sts_f32(s_rel + t * 4,
+                p.rel ? p.rel[static_cast<long long>(h) * (2 * p.L - 1) + (i0 - j0 + p.L - 1) - 127 + t] * kLog2e
+                      : 0.f);
+      if (t < 128) {
+        sts_s32(s_seg + t * 4, p.mask.seg ? p.mask.seg[bl + j0 + t] : 1);
+        sts_s32(s_pos + t * 4, p.mask.pos ? p.mask.pos[bl + j0 + t] : j0 + t);
+      }
+    }
+    named_bar_sync(1, kConsumers);
+    mbar_wait(smem_u32(&kv_full[s]), (it >> 1) & 1);
+    const uint32_t s_k = s_kv + 2 * s * kTile, s_v = s_k + kTile;
+
+    float sv[64];
+#pragma unroll
+    for (int c = 0; c < 64; ++c) sv[c] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+      wgmma_m64n128k16<0, 0>(sv, kdesc(s_q + (kk >> 2) * kChunk + wg * 8192 + (kk & 3) * 32),
+                             kdesc(s_k + (kk >> 2) * kChunk + (kk & 3) * 32), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sv);
+
+    float mloc[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int n = 0; n < 16; ++n) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const int r = wg * 64 + pr0 + 8 * i;       // query row in the tile
+          const int c = n * 8 + cq + j;              // key column in the tile
+          float x = fmaf(sv[4 * n + 2 * i + j], sl2, lds_f32(s_rel + (r - c + 127) * 4));
+          if (!full) {
+            const bool vis = (segq[i] == lds_s32(s_seg + c * 4)) && (segq[i] != 0) &&
+                             (!p.mask.causal || posq[i] >= lds_s32(s_pos + c * 4));
+            x = vis ? x : kMasked;
+          }
+          sv[4 * n + 2 * i + j] = x;
+          mloc[i] = fmaxf(mloc[i], x);
+        }
+      }
+    }
+    float alpha[2], m_new[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      mloc[i] = fmaxf(mloc[i], __shfl_xor_sync(0xffffffffu, mloc[i], 1));
+      mloc[i] = fmaxf(mloc[i], __shfl_xor_sync(0xffffffffu, mloc[i], 2));
+      m_new[i] = fmaxf(m_run[i], mloc[i]);
+      alpha[i] = ex2(m_run[i] - m_new[i]);
+      m_run[i] = m_new[i];
+    }
+    float lsum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int n = 0; n < 16; ++n) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const float p0 = ex2(sv[4 * n + 2 * i] - m_new[i]);
+        const float p1 = ex2(sv[4 * n + 2 * i + 1] - m_new[i]);
+        lsum[i] += p0 + p1;
+        sts_b32(s_pw + sw128_off(pr0 + 8 * i, n * 8 + cq, 8192), pack_bf16x2(p0, p1));
+        o[4 * n + 2 * i] *= alpha[i];
+        o[4 * n + 2 * i + 1] *= alpha[i];
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) l_run[i] = l_run[i] * alpha[i] + lsum[i];
+    fence_proxy_async();          // P (generic-proxy stores) → visible to wgmma's async proxy
+    named_bar_sync(2 + wg, 128);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)                 // O += P·V  (V is MN-major: rows = keys)
+      wgmma_m64n128k16<0, 1>(o, kdesc(s_pw + (kk >> 2) * 8192 + (kk & 3) * 32),
+                             mndesc(s_v + kk * 2048), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&kv_empty[s]));
+    ++it;
+  }
+  // ---- finalize: O / l, log-sum-exp ----
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float l = l_run[i];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = l > 0.f ? 1.f / l : 0.f;      // query block that sees nothing: 0
+    const int qi = i0 + wg * 64 + pr0 + 8 * i;
+    __nv_bfloat16* dst = p.out + ((bl + qi) * p.H + h) * kD;
+#pragma unroll
+    for (int n = 0; n < 16; ++n)
+      *reinterpret_cast<uint32_t*>(dst + n * 8 + cq) =
+          pack_bf16x2(o[4 * n + 2 * i] * inv, o[4 * n + 2 * i + 1] * inv);
+    if ((lane & 3) == 0)
+      p.lse[(static_cast<long long>(b) * p.H + h) * p.L + qi] =
+          l > 0.f ? (m_run[i] + lg2(l)) * kLn2 : 0.f;
   }
 }
 
@@ -463,24 +336,34 @@ struct BwdParams {
   MaskInfo mask;
   const float* lse;      // [B, H, L]
   const float* delta;    // [B, H, L]
-  float* dq_acc;         // [B, L, H, D] fp32, zero-initialised
+  float* dq_part;        // [Jc, B, L, H, D] fp32: dQ of each key block of this launch
   __nv_bfloat16* dk;     // [B, L, H, D]
   __nv_bfloat16* dv;     // [B, L, H, D]
-  float* drel;           // [H, 2L-1] fp32, zero-initialised (or nullptr)
+  float* drel_part;      // [B, H, Jc, 2L-1] fp32, zero-initialised (or nullptr)
   int B, H, L;
+  int j_begin, jc;       // this launch covers key blocks [j_begin, j_begin + jc)
   float scale;
 };
 
 constexpr int kBwdStages = 2;
-// K, V resident + 2 x (Q, dO) + one P/dS tile + 2 KiB of barriers / tables.
-constexpr size_t kBwdSmem = kTile * (2 + 2 * kBwdStages + 1) + 2048 + 1008;
+// K, V resident + 2 x (Q, dO) + one [128 keys x 64 queries] P/dS tile + barriers / tables.
+constexpr size_t kBwdSmem = kTile * (2 + 2 * kBwdStages) + kChunk + 8192 + 1024;
 
+// CTA = (key block, h, b); warpgroup g owns keys [64g, 64g + 64) and keeps dK, dV for them in
+// registers. Every visible query block is processed as two 64-row halves (FlashAttention-2
+// order), with the transposed scores so that P^T / dS^T come out row = key:
+//   S^T = K·Q^T, dP^T = V·dO^T | P^T = exp2(S^T - lse), dS^T = P^T∘(dP^T - delta) |
+//   dV += P^T·dO | dK += dS^T·Q | dQ = dS·K -> this key block's slice of dq_part;
+//   d rel[h, i-j+L-1] += Σ dS along diagonals -> this CTA's row of drel_part.
+// No atomics: the partials are folded in key-block order by the reduce kernels below, so
+// the gradients are identical run to run.
 __global__ void __launch_bounds__(kThreads, 1)
 flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                  const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do,
                  const BwdParams p) {
   const int nblk = p.L / kT;
-  const int j_blk = blockIdx.x;                               // key block (small j = long loop first)
+  const int jrel = blockIdx.x;
+  const int j_blk = p.j_begin + jrel;                         // key block (small j = long loop first)
   const int h = blockIdx.y, b = blockIdx.z;
   const int j0 = j_blk * kT;
   const int4 kmeta = block_meta(p.mask, b, nblk, j_blk);
@@ -491,27 +374,23 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
   const uint32_t s_k = smem_u32(smem);
   const uint32_t s_v = s_k + kTile;
   const uint32_t s_qdo = s_v + kTile;                        // stage s: Q at +2s·kTile, dO behind it
-  const uint32_t s_pds = s_qdo + 2 * kBwdStages * kTile;
-  uint8_t* meta = smem + kTile * (3 + 2 * kBwdStages);
+  const uint32_t s_pds = s_qdo + 2 * kBwdStages * kTile;     // [128 keys x 64 queries], one chunk
+  uint8_t* meta = smem + kTile * (2 + 2 * kBwdStages) + kChunk;
   uint64_t* bars = reinterpret_cast<uint64_t*>(meta);
   uint64_t* kv_bar = bars;
   uint64_t* full_bar = bars + 1;
-  uint64_t* empty_bar = bars + 3;
-  uint64_t* sdp_full = bars + 5;
-  uint64_t* p_ready = bars + 6;
-  uint64_t* p_consumed = bars + 7;
-  uint64_t* ds_ready = bars + 8;
-  uint64_t* dq_full = bars + 9;
-  uint64_t* dq_read = bars + 10;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 11);
+  uint64_t* empty_bar = bars + 1 + kBwdStages;
   const uint32_t s_rel = smem_u32(meta + 128);                // float [256]
-  const uint32_t s_seg = s_rel + 1024;                        // short [128]
-  const uint32_t s_pos = s_seg + 256;                         // short [128]
+  const uint32_t s_seg = s_rel + 1024;                        // int [128]   (query block)
+  const uint32_t s_pos = s_seg + 512;                         // int [128]
+  const uint32_t s_lse = s_pos + 512;                         // float [128] (log2 domain)
+  const uint32_t s_dlt = s_lse + 512;                         // float [128]
+  const uint32_t s_diag = s_dlt + 512;                        // float [256]
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp_idx == 0 && lane == 0) {
+  if (threadIdx.x == kConsumers) {
     tma_prefetch_desc(&map_q);
     tma_prefetch_desc(&map_k);
     tma_prefetch_desc(&map_v);
@@ -519,32 +398,16 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
     mbar_init(smem_u32(kv_bar), 1);
     for (int s = 0; s < kBwdStages; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), 1);
+      mbar_init(smem_u32(&empty_bar[s]), kConsumers / 32);
     }
-    mbar_init(smem_u32(sdp_full), 1);
-    mbar_init(smem_u32(p_ready), 8);
-    mbar_init(smem_u32(p_consumed), 1);
-    mbar_init(smem_u32(ds_ready), 8);
-    mbar_init(smem_u32(dq_full), 1);
-    mbar_init(smem_u32(dq_read), 8);
     fence_barrier_init();
   }
-  if (warp_idx == 1) {
-    tmem_alloc<512>(smem_u32(tmem_ptr_smem));
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const uint32_t t_s = tmem_base;            // S, later dQ tile
-  const uint32_t t_dp = tmem_base + 128;
-  const uint32_t t_dv = tmem_base + 256;
-  const uint32_t t_dk = tmem_base + 384;
 
-  if (warp_idx == 0) {
+  if (warp_idx >= kConsumers / 32) {
     // ============================ TMA producer ============================
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == kConsumers) {
       mbar_arrive_expect_tx(smem_u32(kv_bar), 2 * kTile);
       load_tile(s_k, &map_k, smem_u32(kv_bar), h, j0, b);
       load_tile(s_v, &map_v, smem_u32(kv_bar), h, j0, b);
@@ -560,186 +423,189 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
         ++it;
       }
     }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    // ============================= MMA issuer =============================
-    if (lane == 0) {
-      int n_q = 0;
-      for (int ib = 0; ib < nblk; ++ib)
-        n_q += pair_visible(p.mask, block_meta(p.mask, b, nblk, ib), kmeta) ? 1 : 0;
-      mbar_wait(smem_u32(kv_bar), 0);
-      for (int it = 0; it < n_q; ++it) {
-        const int s = it % kBwdStages;
-        const uint32_t sq = s_qdo + (2 * s) * kTile, sdo = sq + kTile;
-        mbar_wait(smem_u32(&full_bar[s]), (it / kBwdStages) & 1);
-        if (it > 0) mbar_wait(smem_u32(dq_read), (it - 1) & 1);     // dQ tile left columns [0,128)
-        tc_fence_after();
-        issue_gemm<false, false>(t_s, sq, s_k, false);              // S  = Q·K^T
-        issue_gemm<false, false>(t_dp, sdo, s_v, false);            // dP = dO·V^T
-        umma_commit(smem_u32(sdp_full));
-        mbar_wait(smem_u32(p_ready), it & 1);
-        tc_fence_after();
-        issue_gemm<true, true>(t_dv, s_pds, sdo, it > 0);           // dV += P^T·dO
-        umma_commit(smem_u32(p_consumed));
-        mbar_wait(smem_u32(ds_ready), it & 1);
-        tc_fence_after();
-        issue_gemm<true, true>(t_dk, s_pds, sq, it > 0);            // dK += dS^T·Q
-        issue_gemm<false, true>(t_s, s_pds, s_k, false);            // dQ tile = dS·K
-        umma_commit(smem_u32(dq_full));
-        umma_commit(smem_u32(&empty_bar[s]));
-      }
-    }
-    __syncwarp();
-  } else {
-    // ============== softmax-recompute / dS / dQ warps (8 x 32 threads) ==============
-    const int q4 = warp_idx & 3;
-    const int hf = (warp_idx - 2) >> 2;
-    const int r = q4 * 32 + lane;                      // query row (S, dP, dQ) / key row (dK, dV)
-    const int et = (hf * 4 + ((q4 + 2) & 3)) * 32 + lane;
-    const long long bl = static_cast<long long>(b) * p.L;
-    const long long bh = static_cast<long long>(b) * p.H + h;
-    const float sl2 = p.scale * kLog2e;
-    const uint32_t lane_off = static_cast<uint32_t>(q4 * 32) << 16;
-    if (et < 128) {
-      sts_s16(s_seg + et * 2, p.mask.seg ? p.mask.seg[bl + j0 + et] : 1);
-      sts_s16(s_pos + et * 2, p.mask.pos ? p.mask.pos[bl + j0 + et] : j0 + et);
-    }
-
-    int it = 0;
-    for (int ib = 0; ib < nblk; ++ib) {
-      if (!pair_visible(p.mask, block_meta(p.mask, b, nblk, ib), kmeta)) continue;
-      const int i0 = ib * kT;
-      const int i = i0 + r;
-      if (et < 255)
-        sts_f32(s_rel + et * 4,
-                p.rel ? p.rel[static_cast<long long>(h) * (2 * p.L - 1) + (i0 - j0 + p.L - 1) - 127 + et] * kLog2e
-                      : 0.f);
-      const uint32_t rel_a = s_rel + (r + 127) * 4;
-      const int segq = p.mask.seg ? p.mask.seg[bl + i] : 1;
-      const int posq = p.mask.pos ? p.mask.pos[bl + i] : i;
-      const float lse2 = p.lse[bh * p.L + i] * kLog2e;
-      const float delta = p.delta[bh * p.L + i];
-      epi_bar_sync();
-      mbar_wait(smem_u32(sdp_full), it & 1);
-      tc_fence_after();
-      const bool full = pair_full(p.mask, block_meta(p.mask, b, nblk, ib), kmeta);
-      uint32_t dsp[32];                                 // scale·dS, packed bf16x2 (64 values)
-      float a0 = 0.f, a1 = 0.f, a2 = 0.f;               // diagonal sums: lane, lane-32, lane-64
-#pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        uint32_t vs[32], vp[32];
-        tmem_ld_32x32b_x32(t_s + lane_off + hf * 64 + cc * 32, vs);
-        tmem_ld_32x32b_x32(t_dp + lane_off + hf * 64 + cc * 32, vp);
-        tmem_ld_wait();
-        float ds[32];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          uint32_t w[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            float pr[2];
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {
-              const int k = u * 8 + 2 * e + t;
-              const int c = hf * 64 + cc * 32 + k;
-              const float x = fmaf(__uint_as_float(vs[k]), sl2, lds_f32(rel_a - c * 4));
-              const bool vis = full || ((segq == lds_s16(s_seg + c * 2)) && (segq != 0) &&
-                                        (!p.mask.causal || posq >= lds_s16(s_pos + c * 2)));
-              pr[t] = vis ? ex2(x - lse2) : 0.f;
-              ds[k] = pr[t] * (__uint_as_float(vp[k]) - delta);
-            }
-            w[e] = pack_bf16x2(pr[0], pr[1]);
-          }
-          st_shared_v4(s_pds + tile_unit_off(r, hf * 8 + cc * 4 + u), w[0], w[1], w[2], w[3]);
-        }
-        // Toeplitz reduction without smem atomics: lane l takes element k of lane (l+k)%32,
-        // which lies on diagonal (row - col) = r0 - c0 + l  (or l - 32 after the wrap).
-#pragma unroll
-        for (int k = 0; k < 32; ++k) {
-          const float y = __shfl_sync(0xffffffffu, ds[k], (lane + k) & 31);
-          const bool wrap = lane + k >= 32;
-          if (cc == 0) { if (wrap) a1 += y; else a0 += y; }
-          else         { if (wrap) a2 += y; else a1 += y; }
-        }
-#pragma unroll
-        for (int e = 0; e < 16; ++e)
-          dsp[cc * 16 + e] = pack_bf16x2(ds[2 * e] * p.scale, ds[2 * e + 1] * p.scale);
-      }
-      fence_proxy_async();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(p_ready));
-      if (p.drel != nullptr) {
-        // (row - col) of this warp's sub-tile starts at q4*32 - hf*64
-        // index of diagonal (row - col) = q4*32 - hf*64 + lane; the -32 / -64 neighbours of
-        // the outermost lanes are structurally empty and may fall outside [0, 2L-2].
-        const int idx = (i0 - j0) + (p.L - 1) + (q4 * 32 - hf * 64) + lane;
-        float* dr = p.drel + static_cast<long long>(h) * (2 * p.L - 1);
-        if (idx <= 2 * p.L - 2) atomicAdd(dr + idx, a0);
-        if (idx - 32 >= 0) atomicAdd(dr + idx - 32, a1);
-        if (idx - 64 >= 0) atomicAdd(dr + idx - 64, a2);
-      }
-      mbar_wait(smem_u32(p_consumed), it & 1);          // dV MMA has read P: overwrite with dS
-#pragma unroll
-      for (int u = 0; u < 8; ++u)
-        st_shared_v4(s_pds + tile_unit_off(r, hf * 8 + u), dsp[u * 4], dsp[u * 4 + 1],
-                     dsp[u * 4 + 2], dsp[u * 4 + 3]);
-      fence_proxy_async();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(ds_ready));
-      mbar_wait(smem_u32(dq_full), it & 1);
-      tc_fence_after();
-      float* dq = p.dq_acc + ((bl + i) * p.H + h) * kD + hf * 64;
-#pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(t_s + lane_off + hf * 64 + cc * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int e = 0; e < 8; ++e)
-          red_add_v4_f32(dq + cc * 32 + e * 4, __uint_as_float(v[4 * e]), __uint_as_float(v[4 * e + 1]),
-                         __uint_as_float(v[4 * e + 2]), __uint_as_float(v[4 * e + 3]));
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(dq_read));
-      ++it;
-    }
-    // ---- dK, dV: TMEM → bf16 → global (row = key) ----
-    // (the last dq_full commit covers every MMA issued before it, including dV/dK)
-    const long long orow = ((bl + j0 + r) * p.H + h) * kD + hf * 64;
-#pragma unroll
-    for (int which = 0; which < 2; ++which) {
-      const uint32_t t_src = which ? t_dk : t_dv;
-      __nv_bfloat16* dst = (which ? p.dk : p.dv) + orow;
-#pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(t_src + lane_off + hf * 64 + cc * 32, v);
-        tmem_ld_wait();
-        if (it == 0) {                       // no query block sees this key block: zero grads
-#pragma unroll
-          for (int k = 0; k < 32; ++k) v[k] = 0u;
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          int4 w;
-          w.x = pack_bf16x2(__uint_as_float(v[u * 8 + 0]), __uint_as_float(v[u * 8 + 1]));
-          w.y = pack_bf16x2(__uint_as_float(v[u * 8 + 2]), __uint_as_float(v[u * 8 + 3]));
-          w.z = pack_bf16x2(__uint_as_float(v[u * 8 + 4]), __uint_as_float(v[u * 8 + 5]));
-          w.w = pack_bf16x2(__uint_as_float(v[u * 8 + 6]), __uint_as_float(v[u * 8 + 7]));
-          st_v4(dst + cc * 32 + u * 8, w);
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+  // ================= dS / dQ warpgroups (2 x 128 threads) =================
+  setmaxnreg_inc<232>();
+  const int wg = warp_idx >> 2;
+  const int w16 = (warp_idx & 3) * 16 + (lane >> 2);       // fragment row (+ 8 i)
+  const int cq = (lane & 3) * 2;
+  const long long bl = static_cast<long long>(b) * p.L;
+  const long long bh = static_cast<long long>(b) * p.H + h;
+  const float sl2 = p.scale * kLog2e;
+  int segk[2], posk[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int kj = j0 + wg * 64 + w16 + 8 * i;
+    segk[i] = p.mask.seg ? p.mask.seg[bl + kj] : 1;
+    posk[i] = p.mask.pos ? p.mask.pos[bl + kj] : kj;
+  }
+  float dv[64], dk[64];
+#pragma unroll
+  for (int c = 0; c < 64; ++c) { dv[c] = 0.f; dk[c] = 0.f; }
+  mbar_wait(smem_u32(kv_bar), 0);
+
+  int it = 0;
+  for (int ib = 0; ib < nblk; ++ib) {
+    const int4 qmeta = block_meta(p.mask, b, nblk, ib);
+    if (!pair_visible(p.mask, qmeta, kmeta)) continue;
+    const int i0 = ib * kT;
+    const int s = it % kBwdStages;
+    const bool full = pair_full(p.mask, qmeta, kmeta);
+    named_bar_sync(1, kConsumers);                 // previous tables / P-dS tile are free
+    {
+      const int t = threadIdx.x;
+      if (t < 255) {
+        sts_f32(s_rel + t * 4,
+                p.rel ? p.rel[static_cast<long long>(h) * (2 * p.L - 1) + (i0 - j0 + p.L - 1) - 127 + t] * kLog2e
+                      : 0.f);
+        sts_f32(s_diag + t * 4, 0.f);
+      }
+      if (t < 128) {
+        sts_s32(s_seg + t * 4, p.mask.seg ? p.mask.seg[bl + i0 + t] : 1);
+        sts_s32(s_pos + t * 4, p.mask.pos ? p.mask.pos[bl + i0 + t] : i0 + t);
+        sts_f32(s_lse + t * 4, p.lse[bh * p.L + i0 + t] * kLog2e);
+        sts_f32(s_dlt + t * 4, p.delta[bh * p.L + i0 + t]);
+      }
+    }
+    named_bar_sync(1, kConsumers);
+    mbar_wait(smem_u32(&full_bar[s]), (it / kBwdStages) & 1);
+    const uint32_t sq = s_qdo + (2 * s) * kTile, sdo = sq + kTile;
+
+#pragma unroll 1
+    for (int hq = 0; hq < 2; ++hq) {
+      if (hq == 1) named_bar_sync(1, kConsumers);  // both warpgroups' dQ MMAs left the P/dS tile
+      float st[32], dpt[32];   // written by the first MMA of each chain (scale-d = 0)
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)               // S^T = K_g · Q_hq^T
+        wgmma_m64n64k16<0, 0>(st, kdesc(s_k + (kk >> 2) * kChunk + wg * 8192 + (kk & 3) * 32),
+                              kdesc(sq + (kk >> 2) * kChunk + hq * 8192 + (kk & 3) * 32), kk != 0);
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)               // dP^T = V_g · dO_hq^T
+        wgmma_m64n64k16<0, 0>(dpt, kdesc(s_v + (kk >> 2) * kChunk + wg * 8192 + (kk & 3) * 32),
+                              kdesc(sdo + (kk >> 2) * kChunk + hq * 8192 + (kk & 3) * 32), kk != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(st);
+      wgmma_fence_regs(dpt);
+#pragma unroll
+      for (int n = 0; n < 8; ++n) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const int e = 4 * n + 2 * i + j;
+            const int kr = wg * 64 + w16 + 8 * i;    // key row in the tile
+            const int qc = hq * 64 + n * 8 + cq + j; // query column in the tile
+            const float x = fmaf(st[e], sl2, lds_f32(s_rel + (qc - kr + 127) * 4));
+            const bool vis = full || ((lds_s32(s_seg + qc * 4) == segk[i]) && (segk[i] != 0) &&
+                                      (!p.mask.causal || lds_s32(s_pos + qc * 4) >= posk[i]));
+            const float pr = vis ? ex2(x - lds_f32(s_lse + qc * 4)) : 0.f;
+            const float ds = pr * (dpt[e] - lds_f32(s_dlt + qc * 4));
+            st[e] = pr;
+            dpt[e] = ds;
+          }
+        }
+      }
+#pragma unroll
+      for (int n = 0; n < 8; ++n)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+          sts_b32(s_pds + sw128_off(wg * 64 + w16 + 8 * i, n * 8 + cq, kChunk),
+                  pack_bf16x2(st[4 * n + 2 * i], st[4 * n + 2 * i + 1]));
+      fence_proxy_async();
+      named_bar_sync(2 + wg, 128);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)               // dV += P^T_g · dO_hq  (dO MN-major)
+        wgmma_m64n128k16<0, 1>(dv, kdesc(s_pds + wg * 8192 + kk * 32),
+                               mndesc(sdo + hq * 8192 + kk * 2048), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(dv);
+      named_bar_sync(2 + wg, 128);                 // P^T rows of this warpgroup are consumed
+#pragma unroll
+      for (int n = 0; n < 8; ++n)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+          sts_b32(s_pds + sw128_off(wg * 64 + w16 + 8 * i, n * 8 + cq, kChunk),
+                  pack_bf16x2(dpt[4 * n + 2 * i] * p.scale, dpt[4 * n + 2 * i + 1] * p.scale));
+      fence_proxy_async();
+      named_bar_sync(1, kConsumers);               // dQ reads every key row of dS^T
+      float dq[32];            // written by the first dQ MMA (scale-d = 0)
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)               // dK += dS^T_g · Q_hq  (Q MN-major)
+        wgmma_m64n128k16<0, 1>(dk, kdesc(s_pds + wg * 8192 + kk * 32),
+                               mndesc(sq + hq * 8192 + kk * 2048), 1);
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)               // dQ[:, 64g..] = dS · K[:, 64g..]  (both MN-major)
+        wgmma_m64n64k16<1, 1>(dq, mndesc(s_pds + kk * 2048), mndesc(s_k + wg * kChunk + kk * 2048), kk != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(dk);
+      wgmma_fence_regs(dq);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int qi = i0 + hq * 64 + w16 + 8 * i;
+        float* dst = p.dq_part + ((static_cast<long long>(jrel) * p.B * p.L + bl + qi) * p.H + h) * kD +
+                     wg * 64 + cq;
+#pragma unroll
+        for (int n = 0; n < 8; ++n)
+          *reinterpret_cast<float2*>(dst + n * 8) = make_float2(dq[4 * n + 2 * i], dq[4 * n + 2 * i + 1]);
+      }
+      if (p.drel_part != nullptr) {
+        // Fixed-order diagonal sums: each warpgroup's [64 keys x 64 queries] fp32 slab goes
+        // through the free P/dS tile; thread t < 127 sums diagonal (query - key) = t - 63.
+#pragma unroll 1
+        for (int sg = 0; sg < 2; ++sg) {
+          named_bar_sync(1, kConsumers);           // every MMA has left the tile / slab consumed
+          if (wg == sg) {
+#pragma unroll
+            for (int n = 0; n < 8; ++n)
+#pragma unroll
+              for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int j = 0; j < 2; ++j)
+                  sts_f32(s_pds + ((w16 + 8 * i) * 64 + n * 8 + cq + j) * 4, dpt[4 * n + 2 * i + j]);
+          }
+          named_bar_sync(1, kConsumers);
+          const int t = threadIdx.x;
+          if (t < 127) {
+            const int dl = t - 63;
+            float sum = 0.f;
+            for (int kl = max(0, -dl); kl < min(64, 64 - dl); ++kl)
+              sum += lds_f32(s_pds + (kl * 64 + kl + dl) * 4);
+            const uint32_t a = s_diag + (dl + 64 * (hq - sg) + 127) * 4;
+            sts_f32(a, lds_f32(a) + sum);
+          }
+        }
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));
+    if (p.drel_part != nullptr) {
+      // Consecutive query blocks overlap on 127 diagonals; the barrier orders the two adds.
+      named_bar_sync(1, kConsumers);
+      const int t = threadIdx.x;
+      float* dr = p.drel_part + ((bh * p.jc + jrel) * (2 * p.L - 1)) + (i0 - j0) + (p.L - 1) - 127;
+      if (t < 255) dr[t] += lds_f32(s_diag + t * 4);
+    }
+    ++it;
+  }
+  // ---- dK, dV: registers → bf16 → global (row = key); zero when no query sees the block ----
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const long long orow = ((bl + j0 + wg * 64 + w16 + 8 * i) * p.H + h) * kD + cq;
+#pragma unroll
+    for (int n = 0; n < 16; ++n) {
+      *reinterpret_cast<uint32_t*>(p.dv + orow + n * 8) =
+          pack_bf16x2(dv[4 * n + 2 * i], dv[4 * n + 2 * i + 1]);
+      *reinterpret_cast<uint32_t*>(p.dk + orow + n * 8) =
+          pack_bf16x2(dk[4 * n + 2 * i], dk[4 * n + 2 * i + 1]);
+    }
   }
 }
 
@@ -789,6 +655,39 @@ flash_delta_kernel(const __nv_bfloat16* __restrict__ d_o, const __nv_bfloat16* _
 #pragma unroll
   for (int m = 16; m > 0; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
   if (lane == 0) delta[(static_cast<long long>(b) * H + h) * L + l] = s;
+}
+
+// dq_acc[b, l, h, :] += Σ over the launch's key blocks j visible from l's block, in order of j.
+__global__ void __launch_bounds__(256)
+flash_dq_reduce_kernel(const float4* __restrict__ part, float4* __restrict__ dq_acc, MaskInfo mask,
+                       int B, int L, int H, int j_begin, int jc) {
+  const long long n4 = static_cast<long long>(B) * L * H * (kD / 4);
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= n4) return;
+  const long long row = idx / (H * (kD / 4));                 // b * L + l
+  const int b = static_cast<int>(row / L);
+  const int nblk = L / kT;
+  const int4 qm = block_meta(mask, b, nblk, static_cast<int>(row % L) / kT);
+  float4 acc = dq_acc[idx];
+  for (int jr = 0; jr < jc; ++jr) {
+    if (!pair_visible(mask, qm, block_meta(mask, b, nblk, j_begin + jr))) continue;
+    const float4 v = part[static_cast<long long>(jr) * n4 + idx];
+    acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+  }
+  dq_acc[idx] = acc;
+}
+
+// drel[h, t] += Σ_b Σ_j drel_part[b, h, j, t], in order of b, then j.
+__global__ void __launch_bounds__(256)
+flash_drel_reduce_kernel(const float* __restrict__ part, float* __restrict__ drel, int B, int H,
+                         int jc, int n) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  const int h = blockIdx.y;
+  if (t >= n) return;
+  float s = 0.f;
+  for (int b = 0; b < B; ++b)
+    for (int jr = 0; jr < jc; ++jr) s += part[((static_cast<long long>(b) * H + h) * jc + jr) * n + t];
+  drel[static_cast<long long>(h) * n + t] += s;
 }
 
 // dq (bf16) = dq_acc (fp32)
@@ -933,10 +832,8 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
     relc = rel->contiguous();
     p.rel = relc.data_ptr<float>();
   }
-  p.drel = nullptr;
   if (need_drel) {
     drel = torch::zeros({H, 2 * L - 1}, lse.options());
-    p.drel = drel.data_ptr<float>();
   } else {
     drel = torch::empty({0}, lse.options());
   }
@@ -950,7 +847,6 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
   auto dv = torch::empty({B, L, H, kD}, q.options());
   p.lse = lse.data_ptr<float>();
   p.delta = delta.data_ptr<float>();
-  p.dq_acc = dq_acc.data_ptr<float>();
   p.dk = reinterpret_cast<__nv_bfloat16*>(dk.data_ptr());
   p.dv = reinterpret_cast<__nv_bfloat16*>(dv.data_ptr());
   p.B = static_cast<int>(B); p.H = static_cast<int>(H); p.L = static_cast<int>(L);
@@ -965,10 +861,40 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
                                         static_cast<int>(kBwdSmem)));
     configured = true;
   }
-  dim3 grid(static_cast<unsigned>(L / kT), static_cast<unsigned>(H), static_cast<unsigned>(B));
-  flash_bwd_kernel<<<grid, kThreads, kBwdSmem, stream>>>(mq, mkk, mv, mdo, p);
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
-  CountLaunch();
+  // Key blocks go in launches of up to kJChunk; each launch's per-key-block dQ / dRel partials
+  // are folded in key-block order, so the result does not depend on CTA scheduling.
+  constexpr int kJChunk = 8;
+  const int nblk = static_cast<int>(L / kT);
+  const int jc_max = nblk < kJChunk ? nblk : kJChunk;
+  auto dq_part = torch::empty({jc_max, B, L, H, kD}, lse.options());
+  p.dq_part = dq_part.data_ptr<float>();
+  for (int j_begin = 0; j_begin < nblk; j_begin += jc_max) {
+    const int jc = (nblk - j_begin) < jc_max ? (nblk - j_begin) : jc_max;
+    p.j_begin = j_begin;
+    p.jc = jc;
+    torch::Tensor drel_part;
+    p.drel_part = nullptr;
+    if (need_drel) {
+      drel_part = torch::zeros({B, H, jc, 2 * L - 1}, lse.options());
+      p.drel_part = drel_part.data_ptr<float>();
+    }
+    dim3 grid(static_cast<unsigned>(jc), static_cast<unsigned>(H), static_cast<unsigned>(B));
+    flash_bwd_kernel<<<grid, kThreads, kBwdSmem, stream>>>(mq, mkk, mv, mdo, p);
+    C10_CUDA_KERNEL_LAUNCH_CHECK();
+    const long long n4 = B * L * H * (kD / 4);
+    flash_dq_reduce_kernel<<<static_cast<int>((n4 + 255) / 256), 256, 0, stream>>>(
+        reinterpret_cast<const float4*>(p.dq_part), reinterpret_cast<float4*>(dq_acc.data_ptr<float>()),
+        p.mask, p.B, p.L, p.H, j_begin, jc);
+    C10_CUDA_KERNEL_LAUNCH_CHECK();
+    CountLaunch(2);
+    if (need_drel) {
+      const int n = static_cast<int>(2 * L - 1);
+      flash_drel_reduce_kernel<<<dim3((n + 255) / 256, static_cast<unsigned>(H)), 256, 0, stream>>>(
+          p.drel_part, drel.data_ptr<float>(), p.B, p.H, jc, n);
+      C10_CUDA_KERNEL_LAUNCH_CHECK();
+      CountLaunch();
+    }
+  }
   auto dq = torch::empty({B, L, H, kD}, q.options());
   {
     const long long n4 = dq.numel() / 4;

@@ -1,24 +1,24 @@
-// Persistent, warp-specialised bf16 GEMM for sm_100a.
+// Warp-specialised bf16 GEMM for sm_90a (Hopper).
 //
 //   C[g, m, n] = epilogue( sum_k A[g, m, k] * B[g, n, k] )        g in [0, G)
 //
 // * operands are staged by TMA (cp.async.bulk.tensor, 128B swizzle) into a
-//   4-stage shared-memory ring;  either operand may be K-major ([.., MN, K]
+//   4-6 stage shared-memory ring;  either operand may be K-major ([.., MN, K]
 //   storage) or MN-major ([.., K, MN] storage), so the same kernel serves the
 //   forward (x @ w), dgrad (dy @ w^T) and wgrad (x^T @ dy) of every linear /
-//   expert-FFN layer without any transposes in HBM;
-// * one elected thread issues tcgen05.mma (UMMA 128 x BN x 16, fp32 accumulate)
-//   into one of two TMEM accumulator stages (2 x BN columns), so the epilogue of
-//   tile i overlaps the main loop of tile i+1;
-// * four epilogue warps read the accumulator with tcgen05.ld, apply the fused
-//   epilogue (bias, activation, relu-gradient mask / residual add, per-row scale,
-//   accumulate) and store 16-byte vectors straight to global memory.  The store
-//   target of every output row can be redirected through a row-pointer table,
-//   which is how the MoE combine (expert GEMM -> NVLink peer store) is fused.
+//   expert-FFN layer without any transposes in HBM (wgmma reads MN-major bf16
+//   operands through its transpose bits);
+// * two consumer warpgroups each own 64 rows of the 128 x BN tile and issue
+//   wgmma.m64nBNk16 (fp32 accumulators in registers), keeping one k-block of
+//   MMAs in flight while the next stage is awaited;
+// * the fused epilogue (bias, activation, relu-gradient mask / residual add,
+//   per-row scale, accumulate) runs on the accumulator registers and stores
+//   straight to global memory.  The store target of every output row can be
+//   redirected through a row-pointer table, which is how the MoE combine
+//   (expert GEMM -> NVLink peer store) is fused.
 //
-// Grid: one CTA per SM (persistent), 256 threads:
-//   warp 0 = TMA producer, warp 1 = MMA issuer, warp 2 = TMEM allocator,
-//   warps 4..7 = epilogue (TMEM lane quarter = warp_idx % 4).
+// Grid: one CTA per output tile, 288 threads:
+//   warps 0..7 = two consumer warpgroups, warp 8 = TMA producer.
 
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -34,8 +34,9 @@ namespace lb {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;   // 64 bf16 = 128 bytes = one swizzle row
-constexpr int kUmmaK = 16;
-constexpr int kNumThreads = 384;   // warps: 0 TMA, 1 MMA, 2 TMEM alloc, 3 idle, 4-11 epilogue
+constexpr int kMmaK = 16;
+constexpr int kNumConsumers = 256;                 // two warpgroups x 64 rows
+constexpr int kNumThreads = kNumConsumers + 32;    // + one TMA producer warp
 
 enum Act : int { kActNone = 0, kActRelu = 1, kActGelu = 2, kActSilu = 3, kActGeluTanh = 4,
                  kActSquaredRelu = 5 };
@@ -86,121 +87,62 @@ struct EpiRow {
   long long row_off;
   const float* bias;
   float rscale;
-  bool store_ok;
 };
 
-template <int kAct>
-__device__ __forceinline__ void act32(float (&f)[32]) {
-#pragma unroll
-  for (int i = 0; i < 32; ++i) f[i] = apply_act(f[i], kAct);
-}
-
-// One 32-column chunk of one output row: bias / pre-act tap / activation /
-// aux (ReLU-mask or residual add) / row scale / convert / store.
+// One pair of adjacent output columns (col, col + 1) of one row: bias / pre-act tap /
+// activation / aux (ReLU-mask or residual add) / row scale / convert / store.
 template <typename OutT>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const EpiRow& er,
-                                               const uint32_t (&v)[32], int col0) {
-  if (!er.store_ok || col0 >= p.N) return;
-  float f[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]);
+__device__ __forceinline__ void epilogue_pair(const GemmParams& p, const EpiRow& er, float f0,
+                                              float f1, int col) {
   if (er.bias != nullptr) {
-#pragma unroll
-    for (int i = 0; i < 32; i += 4) {
-      if (col0 + i < p.N) {
-        const float4 b = __ldg(reinterpret_cast<const float4*>(er.bias + col0 + i));
-        f[i] += b.x; f[i + 1] += b.y; f[i + 2] += b.z; f[i + 3] += b.w;
-      }
-    }
+    const float2 b = __ldg(reinterpret_cast<const float2*>(er.bias + col));
+    f0 += b.x; f1 += b.y;
   }
   if (p.pre_act != nullptr) {
-    __nv_bfloat16* pr = reinterpret_cast<__nv_bfloat16*>(p.pre_act) + er.row_off + col0;
-#pragma unroll
-    for (int i = 0; i < 32; i += 8) {
-      if (col0 + i < p.N) {
-        int4 o;
-        o.x = pack_bf16x2(f[i], f[i + 1]);
-        o.y = pack_bf16x2(f[i + 2], f[i + 3]);
-        o.z = pack_bf16x2(f[i + 4], f[i + 5]);
-        o.w = pack_bf16x2(f[i + 6], f[i + 7]);
-        st_v4(pr + i, o);
-      }
-    }
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.pre_act) + er.row_off + col) =
+        pack_bf16x2(f0, f1);
   }
-  switch (p.act) {   // hoisted: one uniform branch per chunk, not per element
-    case kActRelu: act32<kActRelu>(f); break;
-    case kActGelu: act32<kActGelu>(f); break;
-    case kActSilu: act32<kActSilu>(f); break;
-    case kActGeluTanh: act32<kActGeluTanh>(f); break;
-    case kActSquaredRelu: act32<kActSquaredRelu>(f); break;
-    default: break;
-  }
+  f0 = apply_act(f0, p.act);
+  f1 = apply_act(f1, p.act);
   if (p.aux_mode != kAuxNone) {
-    const __nv_bfloat16* ax = p.aux + er.row_off + col0;
-    const bool mask = p.aux_mode == kAuxReluMask;
-#pragma unroll
-    for (int i = 0; i < 32; i += 8) {
-      if (col0 + i < p.N) {
-        const int4 a = *reinterpret_cast<const int4*>(ax + i);
-        const uint32_t w[4] = {static_cast<uint32_t>(a.x), static_cast<uint32_t>(a.y),
-                               static_cast<uint32_t>(a.z), static_cast<uint32_t>(a.w)};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float2 t = unpack_bf16x2(w[j]);
-          if (mask) {
-            f[i + 2 * j] = t.x > 0.f ? f[i + 2 * j] : 0.f;
-            f[i + 2 * j + 1] = t.y > 0.f ? f[i + 2 * j + 1] : 0.f;
-          } else {
-            f[i + 2 * j] += t.x;
-            f[i + 2 * j + 1] += t.y;
-          }
-        }
-      }
+    const float2 t = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.aux + er.row_off + col));
+    if (p.aux_mode == kAuxReluMask) {
+      f0 = t.x > 0.f ? f0 : 0.f;
+      f1 = t.y > 0.f ? f1 : 0.f;
+    } else {
+      f0 += t.x;
+      f1 += t.y;
     }
   }
-  if (p.row_scale != nullptr) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) f[i] *= er.rscale;
-  }
+  f0 *= er.rscale;
+  f1 *= er.rscale;
   if constexpr (sizeof(OutT) == 2) {
-    __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(er.c_row) + col0;
-#pragma unroll
-    for (int i = 0; i < 32; i += 8) {
-      if (col0 + i < p.N) {
-        int4 o;
-        o.x = pack_bf16x2(f[i], f[i + 1]);
-        o.y = pack_bf16x2(f[i + 2], f[i + 3]);
-        o.z = pack_bf16x2(f[i + 4], f[i + 5]);
-        o.w = pack_bf16x2(f[i + 6], f[i + 7]);
-        st_v4(out + i, o);
-      }
-    }
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(er.c_row) + col) = pack_bf16x2(f0, f1);
   } else {
-    float* out = reinterpret_cast<float*>(er.c_row) + col0;
-#pragma unroll
-    for (int i = 0; i < 32; i += 4) {
-      if (col0 + i < p.N) {
-        float4 o = make_float4(f[i], f[i + 1], f[i + 2], f[i + 3]);
-        if (p.accumulate) {
-          const float4 old = *reinterpret_cast<const float4*>(out + i);
-          o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
-        }
-        *reinterpret_cast<float4*>(out + i) = o;
-      }
+    float2* out = reinterpret_cast<float2*>(reinterpret_cast<float*>(er.c_row) + col);
+    float2 o = make_float2(f0, f1);
+    if (p.accumulate) {
+      const float2 old = *out;
+      o.x += old.x; o.y += old.y;
     }
+    *out = o;
   }
+}
+
+template <int BN, bool kAK, bool kBK>
+__device__ __forceinline__ void wgmma_bn(float (&acc)[BN / 2], uint64_t adesc, uint64_t bdesc) {
+  if constexpr (BN == 256) wgmma_m64n256k16<kAK ? 0 : 1, kBK ? 0 : 1>(acc, adesc, bdesc, 1);
+  else wgmma_m64n128k16<kAK ? 0 : 1, kBK ? 0 : 1>(acc, adesc, bdesc, 1);
 }
 
 template <int BN, bool kAK, bool kBK, typename OutT>
 __global__ void __launch_bounds__(kNumThreads, 1)
-gemm_tcgen05_kernel(const __grid_constant__ TmapArray tmaps_a,
-                    const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
+gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
+                  const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
   constexpr int kStages = (BN == 256) ? 4 : 6;
   constexpr uint32_t kABytes = kBlockM * kBlockK * 2;   // 16 KiB
   constexpr uint32_t kBBytes = BN * kBlockK * 2;        // 32 KiB (BN=256)
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
-  constexpr uint32_t kTmemCols = 2 * BN;                // two accumulator stages
-  static_assert(kTmemCols <= 512, "TMEM overflow");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024B alignment for SWIZZLE_128B atoms.
@@ -209,183 +151,120 @@ gemm_tcgen05_kernel(const __grid_constant__ TmapArray tmaps_a,
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
-  uint64_t* tmem_full_bar = bars + 2 * kStages;
-  uint64_t* tmem_empty_bar = bars + 2 * kStages + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   const int tiles_m = (p.M + kBlockM - 1) / kBlockM;
-  const int tiles_n = (p.N + BN - 1) / BN;
-  const int tiles_per_group = tiles_m * tiles_n;
-  const int num_tiles = tiles_per_group * p.G;
+  const int tiles_per_group = tiles_m * ((p.N + BN - 1) / BN);
+  const int g = blockIdx.x / tiles_per_group;
+  const int r = blockIdx.x - g * tiles_per_group;
+  const int n_blk = r / tiles_m;
+  const int m_blk = r - n_blk * tiles_m;
+  const int m0 = m_blk * kBlockM, n0 = n_blk * BN;
   const int num_k_blocks = (p.K + kBlockK - 1) / kBlockK;
 
-  if (warp_idx == 0 && lane == 0) {
+  if (threadIdx.x == kNumConsumers) {
     tma_prefetch_desc(&tmaps_a.m[0]);
     tma_prefetch_desc(&tmap_b);
-  }
-  if (warp_idx == 1 && lane == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(smem_u32(&full_bar[i]), 1);
-      mbar_init(smem_u32(&empty_bar[i]), 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&tmem_full_bar[i]), 1);
-      mbar_init(smem_u32(&tmem_empty_bar[i]), 8);
+      mbar_init(smem_u32(&empty_bar[i]), kNumConsumers / 32);
     }
     fence_barrier_init();
   }
-  if (warp_idx == 2) {
-    tmem_alloc<kTmemCols>(smem_u32(tmem_ptr_smem));
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp_idx == 0) {
+  if (warp_idx == kNumConsumers / 32) {
     // ============================ TMA producer ============================
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int g = tile / tiles_per_group;
-        const int r = tile - g * tiles_per_group;
-        const int n_blk = r / tiles_m;
-        const int m_blk = r - n_blk * tiles_m;
-        const int m0 = m_blk * kBlockM, n0 = n_blk * BN;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
-          const uint32_t fb = smem_u32(&full_bar[stage]);
-          mbar_arrive_expect_tx(fb, kStageBytes);
-          const uint32_t sa = smem_u32(smem + stage * kStageBytes);
-          const uint32_t sb = sa + kABytes;
-          const int k0 = kb * kBlockK;
-          const int amap = k0 / p.a_k_per_map;
-          const int ka = k0 - amap * p.a_k_per_map;
-          if constexpr (kAK) {
-            tma_load_3d(sa, &tmaps_a.m[amap], fb, ka, m0, g);
-          } else {
+      for (int kb = 0; kb < num_k_blocks; ++kb) {
+        const int stage = kb % kStages;
+        mbar_wait(smem_u32(&empty_bar[stage]), ((kb / kStages) & 1) ^ 1);
+        const uint32_t fb = smem_u32(&full_bar[stage]);
+        mbar_arrive_expect_tx(fb, kStageBytes);
+        const uint32_t sa = smem_u32(smem + stage * kStageBytes);
+        const uint32_t sb = sa + kABytes;
+        const int k0 = kb * kBlockK;
+        const int amap = k0 / p.a_k_per_map;
+        const int ka = k0 - amap * p.a_k_per_map;
+        if constexpr (kAK) {
+          tma_load_3d(sa, &tmaps_a.m[amap], fb, ka, m0, g);
+        } else {
 #pragma unroll
-            for (int i = 0; i < kBlockM / 64; ++i)
-              tma_load_3d(sa + i * (64 * kBlockK * 2), &tmaps_a.m[amap], fb, m0 + 64 * i, ka, g);
-          }
-          if constexpr (kBK) {
-            tma_load_3d(sb, &tmap_b, fb, k0, n0, g);
-          } else {
+          for (int i = 0; i < kBlockM / 64; ++i)
+            tma_load_3d(sa + i * (64 * kBlockK * 2), &tmaps_a.m[amap], fb, m0 + 64 * i, ka, g);
+        }
+        if constexpr (kBK) {
+          tma_load_3d(sb, &tmap_b, fb, k0, n0, g);
+        } else {
 #pragma unroll
-            for (int i = 0; i < BN / 64; ++i)
-              tma_load_3d(sb + i * (64 * kBlockK * 2), &tmap_b, fb, n0 + 64 * i, k0, g);
-          }
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
+          for (int i = 0; i < BN / 64; ++i)
+            tma_load_3d(sb + i * (64 * kBlockK * 2), &tmap_b, fb, n0 + 64 * i, k0, g);
         }
       }
     }
-    __syncwarp();
-  } else if (warp_idx == 1) {
-    // ============================= MMA issuer =============================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(1, 1, !kAK, !kBK, kBlockM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(smem_u32(&tmem_empty_bar[acc]), acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          mbar_wait(smem_u32(&full_bar[stage]), phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * kStageBytes);
-          const uint32_t sb = sa + kABytes;
-#pragma unroll
-          for (int j = 0; j < kBlockK / kUmmaK; ++j) {
-            // K-major: advance 32 B inside the 128 B swizzle row.
-            // MN-major: advance 16 K-rows of 128 B; 64-wide MN chunks are
-            //           64*kBlockK*2 bytes apart (LBO), 8-row groups 1 KiB (SBO).
-            const uint64_t adesc =
-                kAK ? make_smem_desc_sw128(sa + j * 32, 16, 1024)
-                    : make_smem_desc_sw128(sa + j * (kUmmaK * 128), 64 * kBlockK * 2, 1024);
-            const uint64_t bdesc =
-                kBK ? make_smem_desc_sw128(sb + j * 32, 16, 1024)
-                    : make_smem_desc_sw128(sb + j * (kUmmaK * 128), 64 * kBlockK * 2, 1024);
-            umma_f16(tmem_d, adesc, bdesc, idesc, (kb | j) != 0 ? 1u : 0u);
-          }
-          umma_commit(smem_u32(&empty_bar[stage]));   // frees the smem slot when MMAs retire
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(smem_u32(&tmem_full_bar[acc]));   // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-    __syncwarp();
-  } else if (warp_idx >= 4) {
-    // ============================== epilogue ==============================
-    // 8 warps: warp w owns TMEM lanes 32*(w%4).. and one half of the tile's columns.
-    const int q = warp_idx & 3;                 // TMEM lane quarter
-    const int half = (warp_idx - 4) >> 2;       // column half
-    constexpr int kChunks = BN / 64;            // 32-column chunks per warp
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int g = tile / tiles_per_group;
-      const int r = tile - g * tiles_per_group;
-      const int n_blk = r / tiles_m;
-      const int m_blk = r - n_blk * tiles_m;
-      const int row = m_blk * kBlockM + q * 32 + lane;
-      const int n0 = n_blk * BN;
-      const bool row_ok = row < p.M;
-
-      EpiRow er;
-      er.row_off = static_cast<long long>(g) * p.c_batch + static_cast<long long>(row) * p.ldc;
-      if (p.row_ptrs != nullptr && row_ok) {
-        er.c_row = p.row_ptrs[static_cast<long long>(g) * p.M + row];
-      } else if (p.nblk_ptrs != nullptr) {
-        er.c_row = reinterpret_cast<OutT*>(p.nblk_ptrs[n_blk]) + static_cast<long long>(row) * p.ldc - n0;
-      } else {
-        er.c_row = reinterpret_cast<OutT*>(p.c) + er.row_off;
-      }
-      er.store_ok = row_ok && (er.c_row != nullptr);
-      er.rscale = (p.row_scale != nullptr && row_ok)
-                      ? p.row_scale[static_cast<long long>(g) * p.M + row] : 1.f;
-      er.bias = p.bias ? p.bias + static_cast<long long>(g) * p.N : nullptr;
-
-      mbar_wait(smem_u32(&tmem_full_bar[acc]), acc_phase);
-      tc_fence_after();
-
-      // Software-pipelined TMEM reads: chunk c+1 is in flight while chunk c is
-      // converted and stored.
-      const uint32_t tbase = tmem_base + acc * BN + half * (BN / 2) +
-                             (static_cast<uint32_t>(q * 32) << 16);
-      const int cbase = n0 + half * (BN / 2);
-      uint32_t va[32], vb[32];
-      tmem_ld_32x32b_x32(tbase, va);
-#pragma unroll 1
-      for (int c = 0; c < kChunks; c += 2) {
-        tmem_ld_wait();
-        tmem_ld_32x32b_x32(tbase + (c + 1) * 32, vb);
-        epilogue_chunk<OutT>(p, er, va, cbase + c * 32);
-        tmem_ld_wait();
-        if (c + 2 < kChunks) tmem_ld_32x32b_x32(tbase + (c + 2) * 32, va);
-        epilogue_chunk<OutT>(p, er, vb, cbase + (c + 1) * 32);
-      }
-      // Release this accumulator stage back to the MMA warp.
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&tmem_empty_bar[acc]));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc<kTmemCols>(tmem_base);
+  // ============================== consumers ==============================
+  // Warpgroup wg owns tile rows [64 wg, 64 wg + 64). Its A rows start 8 KiB into the
+  // stage for both majors: 64 K-major rows of 128 B, or the wg-th 64-wide MN chunk.
+  const int wg = warp_idx >> 2;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  for (int kb = 0; kb < num_k_blocks; ++kb) {
+    const int stage = kb % kStages;
+    mbar_wait(smem_u32(&full_bar[stage]), (kb / kStages) & 1);
+    const uint32_t sa = smem_u32(smem + stage * kStageBytes) + wg * (64 * 128);
+    const uint32_t sb = smem_u32(smem + stage * kStageBytes) + kABytes;
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < kBlockK / kMmaK; ++j) {
+      // K-major: advance 32 B inside the 128 B swizzle row.
+      // MN-major: advance 16 K-rows of 128 B; 64-wide MN chunks are
+      //           64*kBlockK*2 bytes apart (LBO), 8-row groups 1 KiB (SBO).
+      const uint64_t adesc =
+          kAK ? make_smem_desc_sw128(sa + j * 32, 16, 1024)
+              : make_smem_desc_sw128(sa + j * (kMmaK * 128), 64 * kBlockK * 2, 1024);
+      const uint64_t bdesc =
+          kBK ? make_smem_desc_sw128(sb + j * 32, 16, 1024)
+              : make_smem_desc_sw128(sb + j * (kMmaK * 128), 64 * kBlockK * 2, 1024);
+      wgmma_bn<BN, kAK, kBK>(acc, adesc, bdesc);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();                 // the previous k-block's MMAs have retired
+    __syncwarp();
+    if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[(kb - 1) % kStages]));
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+
+  // ============================== epilogue ==============================
+  const int wrow = m0 + wg * 64 + (warp_idx & 3) * 16 + (lane >> 2);
+  const int cq = (lane & 3) * 2;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = wrow + 8 * i;
+    if (row >= p.M) continue;
+    EpiRow er;
+    er.row_off = static_cast<long long>(g) * p.c_batch + static_cast<long long>(row) * p.ldc;
+    if (p.row_ptrs != nullptr) {
+      er.c_row = p.row_ptrs[static_cast<long long>(g) * p.M + row];
+    } else if (p.nblk_ptrs != nullptr) {
+      er.c_row = reinterpret_cast<OutT*>(p.nblk_ptrs[n_blk]) + static_cast<long long>(row) * p.ldc - n0;
+    } else {
+      er.c_row = reinterpret_cast<OutT*>(p.c) + er.row_off;
+    }
+    if (er.c_row == nullptr) continue;
+    er.rscale = p.row_scale != nullptr ? p.row_scale[static_cast<long long>(g) * p.M + row] : 1.f;
+    er.bias = p.bias ? p.bias + static_cast<long long>(g) * p.N : nullptr;
+#pragma unroll
+    for (int n = 0; n < BN / 8; ++n) {
+      const int col = n0 + n * 8 + cq;
+      if (col < p.N) epilogue_pair<OutT>(p, er, acc[4 * n + 2 * i], acc[4 * n + 2 * i + 1], col);
+    }
   }
 }
 
@@ -434,10 +313,10 @@ CUtensorMap MakeMap(const void* base, int64_t inner, int64_t rows, int64_t group
 
 template <int BN, bool kAK, bool kBK, typename OutT>
 static void Launch(const TmapArray& ta, const CUtensorMap& tb, const GemmParams& p,
-                   cudaStream_t stream, int num_sms) {
+                   cudaStream_t stream) {
   constexpr int kStages = (BN == 256) ? 4 : 6;
   constexpr size_t smem = kStages * (kBlockM * kBlockK * 2 + BN * kBlockK * 2) + 1024 + 256;
-  auto kern = gemm_tcgen05_kernel<BN, kAK, kBK, OutT>;
+  auto kern = gemm_wgmma_kernel<BN, kAK, kBK, OutT>;
   static bool configured = false;
   if (!configured) {
     C10_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -445,25 +324,22 @@ static void Launch(const TmapArray& ta, const CUtensorMap& tb, const GemmParams&
     configured = true;
   }
   const int tiles = p.G * ((p.M + kBlockM - 1) / kBlockM) * ((p.N + BN - 1) / BN);
-  const int grid = tiles < num_sms ? tiles : num_sms;
-  kern<<<grid, kNumThreads, smem, stream>>>(ta, tb, p);
+  kern<<<tiles, kNumThreads, smem, stream>>>(ta, tb, p);
   CountLaunch();
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
 template <int BN, typename OutT>
 static void Dispatch(bool ak, bool bk, const TmapArray& ta, const CUtensorMap& tb,
-                     const GemmParams& p, cudaStream_t s, int sms) {
-  if (ak && bk) Launch<BN, true, true, OutT>(ta, tb, p, s, sms);
-  else if (ak && !bk) Launch<BN, true, false, OutT>(ta, tb, p, s, sms);
-  else if (!ak && bk) Launch<BN, false, true, OutT>(ta, tb, p, s, sms);
-  else Launch<BN, false, false, OutT>(ta, tb, p, s, sms);
+                     const GemmParams& p, cudaStream_t s) {
+  if (ak && bk) Launch<BN, true, true, OutT>(ta, tb, p, s);
+  else if (ak && !bk) Launch<BN, true, false, OutT>(ta, tb, p, s);
+  else if (!ak && bk) Launch<BN, false, true, OutT>(ta, tb, p, s);
+  else Launch<BN, false, false, OutT>(ta, tb, p, s);
 }
 
-// Wave-quantisation heuristic switch. Off by default: measured on B200
-// (profiles/gemm_bn_probe_r1.jsonl) the 128-wide tile runs at ≈75 % of the 256-wide tile's
-// per-FLOP rate (operand traffic per FLOP is 1.33× higher), which costs more than the
-// 3.46 → 4 wave rounding it avoids. LINGVO_B200_GEMM_AUTO_BN=1 turns it on for experiments.
+// Wave-quantisation heuristic switch, off by default: the 128-wide tile moves 1.33x more
+// operand bytes per FLOP than the 256-wide one. LINGVO_B200_GEMM_AUTO_BN=1 turns it on.
 static bool GemmAutoBn128() {
   static const bool on = [] {
     const char* e = getenv("LINGVO_B200_GEMM_AUTO_BN");
@@ -596,8 +472,8 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
   if (M == 0 || N == 0 || G == 0) return out;
 
   // Tile-N: 256 unless N is small — or unless 128-wide tiles quantise better onto the SMs:
-  // an [8192, 2048] output is 512 tiles of 128×256 = 3.46 waves on 148 SMs (4 are paid for),
-  // but 1024 tiles of 128×128 = 6.92 half-cost waves. LINGVO_B200_GEMM_BN=128|256 forces one.
+  // an [8192, 2048] output is 512 tiles of 128×256 = 3.88 waves on 132 SMs (4 are paid for),
+  // but 1024 tiles of 128×128 = 7.76 half-cost waves. LINGVO_B200_GEMM_BN=128|256 forces one.
   bool bn256 = N > 128;
   if (bn256) {
     static const int forced = [] {
@@ -638,13 +514,12 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
       : MakeMap(b.data_ptr(), N, Kb, G, b.stride(1), G > 1 ? b.stride(0) : b.stride(1) * b.size(1), kBlockK);
 
   cudaStream_t stream = at::cuda::getCurrentCUDAStream();
-  const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
   if (bn256) {
-    if (fp32) Dispatch<256, float>(a_kmajor, b_kmajor, ta, tb, p, stream, sms);
-    else Dispatch<256, __nv_bfloat16>(a_kmajor, b_kmajor, ta, tb, p, stream, sms);
+    if (fp32) Dispatch<256, float>(a_kmajor, b_kmajor, ta, tb, p, stream);
+    else Dispatch<256, __nv_bfloat16>(a_kmajor, b_kmajor, ta, tb, p, stream);
   } else {
-    if (fp32) Dispatch<128, float>(a_kmajor, b_kmajor, ta, tb, p, stream, sms);
-    else Dispatch<128, __nv_bfloat16>(a_kmajor, b_kmajor, ta, tb, p, stream, sms);
+    if (fp32) Dispatch<128, float>(a_kmajor, b_kmajor, ta, tb, p, stream);
+    else Dispatch<128, __nv_bfloat16>(a_kmajor, b_kmajor, ta, tb, p, stream);
   }
   return out;
 }

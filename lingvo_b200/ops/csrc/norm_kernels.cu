@@ -8,7 +8,7 @@
 // dscale / dbias with one atomicAdd per column per CTA.
 //
 // One warp owns a row; 16-byte vector loads; rows are streamed by a persistent
-// grid (148 SMs x 8 CTAs). Memory-bound: forward reads x (+res) once and writes
+// grid (132 SMs x 8 CTAs). Memory-bound: forward reads x (+res) once and writes
 // y (+sum) once; backward reads x, dy once and writes dx once.
 
 #include <ATen/cuda/CUDAContext.h>

@@ -10,6 +10,9 @@
 //   D  apply   : w -= g*fr*fc * max(rms(w), eps2)*lr / max(1, rms(x)/clip);
 //                bf16 copy of w written alongside.
 // HBM traffic ~ 3 reads of g + read/write of w + write of the bf16 copy.
+// Sums that span CTAs (row sums across column chunks, Σg², Σw², the clipping RMS) are
+// written as per-CTA / per-warp partials and folded in a fixed order, never by float
+// atomics, so the same inputs give bit-identical updates on every run.
 //
 // adam_flat: elementwise Adam on a flat fp32 shard with grad scale and bf16
 // copy-out — the update half of the fused reduce-scatter + partitioned Adam.
@@ -89,8 +92,8 @@ template <typename GT>
 __global__ void __launch_bounds__(kWarps * 32)
 adafactor_stats_kernel(const GT* __restrict__ g, const float* __restrict__ w,
                        float* __restrict__ rowsum, float* __restrict__ colpart,
-                       float* __restrict__ acc, int B, int R, int C, int nblk, int nchunk,
-                       int with_w, float* __restrict__ total_sumsq, long long ldg) {
+                       float* __restrict__ rowpart, float* __restrict__ bpart, int B, int R,
+                       int C, int nblk, int nchunk, int with_w, long long ldg) {
   // ldg: row stride of g in elements (== C unless g is a column slice of a wider matrix;
   // strided gradients are only accepted for B == 1).
   // with_w: also accumulate sum(w^2) (only on the first step of a variable; later
@@ -175,21 +178,21 @@ adafactor_stats_kernel(const GT* __restrict__ g, const float* __restrict__ w,
 #pragma unroll
     for (int k = 0; k < kWarps; ++k) s += rpart[k][lane];
     if (lane < nrows) {
-      float* dst = rowsum + static_cast<size_t>(b) * R + r0 + lane;
-      if (nchunk == 1) *dst = s;
-      else atomicAdd(dst, s);
+      const size_t ri = static_cast<size_t>(b) * R + r0 + lane;
+      if (nchunk == 1) rowsum[ri] = s;
+      else rowpart[static_cast<size_t>(chunk) * B * R + ri] = s;   // folded in chunk order
     } else {
       s = 0.f;
     }
     const float tg = warp_sum(s);
     if (lane == 0) {
-      if (total_sumsq != nullptr && tg != 0.f) atomicAdd(total_sumsq, tg);
+      float tw = 0.f;
       if (with_w) {
-        float tw = 0.f;
 #pragma unroll
         for (int k = 0; k < kWarps; ++k) tw += wpart[k];
-        atomicAdd(&acc[0], tw);
       }
+      bpart[2 * blockIdx.x] = tg;        // Σg², Σw² of this CTA, folded in CTA order
+      bpart[2 * blockIdx.x + 1] = tw;
     }
   }
 }
@@ -277,7 +280,7 @@ __global__ void adafactor_factors_kernel(float* __restrict__ vr, float* __restri
 template <typename GT>
 __global__ void __launch_bounds__(kWarps * 32)
 adafactor_rms_kernel(const GT* __restrict__ g, const float* __restrict__ fr,
-                     const float* __restrict__ fc, float* __restrict__ acc, int B, int R, int C,
+                     const float* __restrict__ fc, float* __restrict__ wpart, int B, int R, int C,
                      int items, const float* __restrict__ gscale, long long ldg) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float gs = gscale ? *gscale : 1.f;
@@ -319,14 +322,15 @@ adafactor_rms_kernel(const GT* __restrict__ g, const float* __restrict__ fr,
     }
   }
   s = warp_sum(s);
-  if (lane == 0) atomicAdd(&acc[1], s);
+  if (lane == 0) wpart[blockIdx.x * kWarps + warp] = s;
 }
 
 template <typename GT>
 __global__ void __launch_bounds__(kWarps * 32)
 adafactor_apply_kernel(const GT* __restrict__ g, float* __restrict__ w,
                        __nv_bfloat16* __restrict__ w_bf16, const float* __restrict__ fr,
-                       const float* __restrict__ fc, const float* __restrict__ acc, int B, int R,
+                       const float* __restrict__ fc, const float* __restrict__ acc,
+                       float* __restrict__ wpart, int B, int R,
                        int C, float lr, float eps2, float clip, int mult_by_param_scale,
                        float numel, int items, const float* __restrict__ gscale,
                        const float* __restrict__ hyper, long long ldg) {
@@ -387,7 +391,7 @@ adafactor_apply_kernel(const GT* __restrict__ g, float* __restrict__ w,
     }
   }
   wsq = warp_sum(wsq);                       // sum(w_new^2): next step's parameter scale
-  if (lane == 0) atomicAdd(const_cast<float*>(&acc[2]), wsq);
+  if (lane == 0) wpart[blockIdx.x * kWarps + warp] = wsq;
 }
 
 template <typename GT>
@@ -495,7 +499,7 @@ adafactor_small_kernel(const SmallVar* __restrict__ table, float lr, float decay
 
 // Σg² and Σw² over every variable of a SmallVar table: one CTA per variable, two adds.
 __global__ void __launch_bounds__(256)
-small_sumsq_kernel(const SmallVar* __restrict__ table, float* __restrict__ out) {
+small_sumsq_kernel(const SmallVar* __restrict__ table, float* __restrict__ bpart) {
   __shared__ float red[2][8];
   const SmallVar sv = table[blockIdx.x];
   const float* w = reinterpret_cast<const float*>(sv.w);
@@ -522,9 +526,41 @@ small_sumsq_kernel(const SmallVar* __restrict__ table, float* __restrict__ out) 
       tg += red[0][k];
       tw += red[1][k];
     }
-    atomicAdd(&out[0], tg);
-    atomicAdd(&out[1], tw);
+    bpart[2 * blockIdx.x] = tg;
+    bpart[2 * blockIdx.x + 1] = tw;
   }
+}
+
+// dst[0] += Σ_i part[i * stride] in a fixed order (one CTA): the per-CTA / per-warp partial
+// sums above are combined here instead of by atomics, so every step sums in the same order.
+__global__ void __launch_bounds__(256)
+ordered_sum_kernel(const float* __restrict__ part, int count, int stride, float* __restrict__ dst) {
+  __shared__ float red[256];
+  float s = 0.f;
+  for (int i = threadIdx.x; i < count; i += 256) s += part[static_cast<size_t>(i) * stride];
+  red[threadIdx.x] = s;
+  __syncthreads();
+  for (int off = 128; off > 0; off >>= 1) {
+    if (threadIdx.x < off) red[threadIdx.x] += red[threadIdx.x + off];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) dst[0] += red[0];
+}
+
+// dst[x] = Σ_c part[c * n + x], c in order.
+__global__ void __launch_bounds__(256)
+chunk_sum_kernel(const float* __restrict__ part, int nchunk, long long n, float* __restrict__ dst) {
+  const long long x = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (x >= n) return;
+  float s = 0.f;
+  for (int c = 0; c < nchunk; ++c) s += part[c * n + x];
+  dst[x] = s;
+}
+
+static void OrderedSum(const float* part, int count, int stride, float* dst, cudaStream_t stream) {
+  ordered_sum_kernel<<<1, 256, 0, stream>>>(part, count, stride, dst);
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  CountLaunch();
 }
 
 struct AfLayout {
@@ -620,16 +656,29 @@ void adafactor_stats(const torch::Tensor& w, const torch::Tensor& g, torch::Tens
   const int nblk = static_cast<int>((R + kStatRows - 1) / kStatRows);
   const int nchunk = static_cast<int>((C + kStatCols - 1) / kStatCols);
   float* colpart = ColPartials(w.device(), stream.stream(), slot, B * nblk * C);
-  if (nchunk > 1)
-    C10_CUDA_CHECK(cudaMemsetAsync(l.rowsum, 0, sizeof(float) * l.br4, stream));
+  const int grid = static_cast<int>(B) * nblk * nchunk;
+  auto fopt = w.options().dtype(torch::kFloat32);
+  auto bpart = torch::empty({grid, 2}, fopt);
+  torch::Tensor rowpart;
+  if (nchunk > 1) rowpart = torch::empty({nchunk, B * R}, fopt);
   auto run = [&](auto tag) {
     using GT = decltype(tag);
-    adafactor_stats_kernel<GT><<<static_cast<int>(B) * nblk * nchunk, kWarps * 32, 0, stream>>>(
-        reinterpret_cast<const GT*>(g.data_ptr()), w.data_ptr<float>(), l.rowsum, colpart, l.acc,
-        (int)B, (int)R, (int)C, nblk, nchunk, with_w, tot, (long long)ldg);
+    adafactor_stats_kernel<GT><<<grid, kWarps * 32, 0, stream>>>(
+        reinterpret_cast<const GT*>(g.data_ptr()), w.data_ptr<float>(), l.rowsum, colpart,
+        rowpart.defined() ? rowpart.data_ptr<float>() : nullptr, bpart.data_ptr<float>(),
+        (int)B, (int)R, (int)C, nblk, nchunk, with_w, (long long)ldg);
   };
   if (g.scalar_type() == torch::kBFloat16) run(__nv_bfloat16());
   else { TORCH_CHECK(g.scalar_type() == torch::kFloat32); run(float()); }
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+  if (nchunk > 1) {
+    chunk_sum_kernel<<<static_cast<int>((B * R + 255) / 256), 256, 0, stream>>>(
+        rowpart.data_ptr<float>(), nchunk, B * R, l.rowsum);
+    C10_CUDA_KERNEL_LAUNCH_CHECK();
+    CountLaunch();
+  }
+  if (tot != nullptr) OrderedSum(bpart.data_ptr<float>(), grid, 2, tot, stream);
+  if (with_w) OrderedSum(bpart.data_ptr<float>() + 1, grid, 2, l.acc, stream);
   adafactor_colreduce_kernel<<<dim3(static_cast<unsigned>((C + 255) / 256),
                                     static_cast<unsigned>(B)), 256, 0, stream>>>(
       colpart, l.colsum, (int)C, nblk);
@@ -662,16 +711,22 @@ void adafactor_update(torch::Tensor w, const torch::Tensor& g, torch::Tensor vr,
       vr.data_ptr<float>(), vc.data_ptr<float>(), l.rowsum, l.colsum, l.fr, l.fc, (int)B, (int)R,
       (int)C, (float)decay, vr_is_rows ? 1 : 0, l.acc,
       (recompute_wsq || !mult_by_param_scale) ? 1 : 0, gsp, (float)eps1, hp);
+  auto wpart = torch::empty({2, l.grid * kWarps}, w.options().dtype(torch::kFloat32));
+  float* wp_rms = wpart.data_ptr<float>();
+  float* wp_apply = wp_rms + l.grid * kWarps;
   auto run = [&](auto tag) {
     using GT = decltype(tag);
     const GT* gp = reinterpret_cast<const GT*>(g.data_ptr());
-    if (clip > 0)
+    if (clip > 0) {
       adafactor_rms_kernel<GT><<<l.grid, kWarps * 32, 0, stream>>>(
-          gp, l.fr, l.fc, l.acc, (int)B, (int)R, (int)C, l.items, gsp, (long long)ldg);
+          gp, l.fr, l.fc, wp_rms, (int)B, (int)R, (int)C, l.items, gsp, (long long)ldg);
+      OrderedSum(wp_rms, l.grid * kWarps, 1, l.acc + 1, stream);
+    }
     adafactor_apply_kernel<GT><<<l.grid, kWarps * 32, 0, stream>>>(
-        gp, w.data_ptr<float>(), wb, l.fr, l.fc, l.acc, (int)B, (int)R, (int)C, (float)lr,
-        (float)eps2, (float)clip, mult_by_param_scale ? 1 : 0, numel, l.items, gsp, hp,
+        gp, w.data_ptr<float>(), wb, l.fr, l.fc, l.acc, wp_apply, (int)B, (int)R, (int)C,
+        (float)lr, (float)eps2, (float)clip, mult_by_param_scale ? 1 : 0, numel, l.items, gsp, hp,
         (long long)ldg);
+    OrderedSum(wp_apply, l.grid * kWarps, 1, l.acc + 2, stream);
   };
   if (g.scalar_type() == torch::kBFloat16) run(__nv_bfloat16());
   else { TORCH_CHECK(g.scalar_type() == torch::kFloat32); run(float()); }
@@ -707,9 +762,13 @@ void small_sumsq(const torch::Tensor& table, torch::Tensor out) {
   const int n = static_cast<int>(table.size(0));
   if (n == 0) return;
   const c10::cuda::CUDAGuard guard(table.device());
-  small_sumsq_kernel<<<n, 256, 0, at::cuda::getCurrentCUDAStream()>>>(
-      reinterpret_cast<const SmallVar*>(table.data_ptr<int64_t>()), out.data_ptr<float>());
+  auto stream = at::cuda::getCurrentCUDAStream();
+  auto bpart = torch::empty({n, 2}, out.options());
+  small_sumsq_kernel<<<n, 256, 0, stream>>>(
+      reinterpret_cast<const SmallVar*>(table.data_ptr<int64_t>()), bpart.data_ptr<float>());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
+  OrderedSum(bpart.data_ptr<float>(), n, 2, out.data_ptr<float>(), stream);
+  OrderedSum(bpart.data_ptr<float>() + 1, n, 2, out.data_ptr<float>() + 1, stream);
   CountLaunch();
 }
 

@@ -1,7 +1,7 @@
-// Thin inline-PTX wrappers for the sm_100a features used by lingvo_b200
-// kernels: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit
-// / ld / fences) and a few cache-hinted / system-scope memory ops used by the
-// NVLink peer-memory kernels.  No CUTLASS dependency.
+// Thin inline-PTX wrappers for the sm_90a (Hopper) features used by lingvo_b200
+// kernels: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma) and a few
+// cache-hinted / system-scope memory ops used by the NVLink peer-memory kernels.
+// No CUTLASS dependency.
 #pragma once
 
 #include <cuda.h>
@@ -98,101 +98,111 @@ __device__ __forceinline__ void tma_store_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// -------------------------------------------------------------- tcgen05 ----
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-               ::"r"(dst_smem), "n"(kCols)
-               : "memory");
+// ---------------------------------------------------------------- wgmma ----
+// Warpgroup MMA (sm_90a): four consecutive warps, starting at a warp index that is a
+// multiple of four, issue each wgmma together. Accumulators live in registers; the
+// fragment of thread t (warp w = t/32 of the warpgroup, lane l) for an m64nN tile holds
+//   d[4n + 2i + j] = D[16w + l/4 + 8i][8n + 2(l%4) + j],  n < N/8, i, j in {0, 1}.
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr),
-               "n"(kCols)
-               : "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16/fp16 inputs.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n"
-      ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// fp8 (e4m3/e5m2) inputs, fp32 accumulate (no block scaling).
-__device__ __forceinline__ void umma_f8f6f4(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n"
-      "}\n"
-      ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued MMAs have completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-      ::"r"(bar)
-      : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread.
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "[%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]),
-        "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]),
-        "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]),
-        "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// Eight consecutive accumulator registers as read-write asm operands.
+#define LB_ACC8(o)                                                                      \
+  "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), \
+      "+f"(d[o + 6]), "+f"(d[o + 7])
+// Keeps the compiler from moving accumulator reads / writes across a wgmma in flight.
+template <int kN>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[kN]) {
+#pragma unroll
+  for (int i = 0; i < kN; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-//  [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1
-//  [61,64) layout type (2 = SWIZZLE_128B)
+// D[64 x 64] (+)= A[64 x 16] * B[16 x 64], both operands in shared memory.
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc,
+                                              int scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, %35, %36;\n"
+      "}\n"
+      : LB_ACC8(0), LB_ACC8(8), LB_ACC8(16), LB_ACC8(24)
+      : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(kTransA), "n"(kTransB));
+}
+
+// D[64 x 128] (+)= A[64 x 16] * B[16 x 128], both operands in shared memory.
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc,
+                                              int scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n"
+      "}\n"
+      : LB_ACC8(0), LB_ACC8(8), LB_ACC8(16), LB_ACC8(24), LB_ACC8(32), LB_ACC8(40), LB_ACC8(48), LB_ACC8(56)
+      : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(kTransA), "n"(kTransB));
+}
+
+// D[64 x 256] (+)= A[64 x 16] * B[16 x 256], both operands in shared memory.
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t adesc, uint64_t bdesc,
+                                              int scale_d) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, %131, %132;\n"
+      "}\n"
+      : LB_ACC8(0), LB_ACC8(8), LB_ACC8(16), LB_ACC8(24), LB_ACC8(32), LB_ACC8(40), LB_ACC8(48), LB_ACC8(56), LB_ACC8(64), LB_ACC8(72), LB_ACC8(80), LB_ACC8(88), LB_ACC8(96), LB_ACC8(104), LB_ACC8(112), LB_ACC8(120)
+      : "l"(adesc), "l"(bdesc), "r"(scale_d), "n"(kTransA), "n"(kTransB));
+}
+
+// Shared-memory matrix descriptor (sm_90 wgmma layout):
+//  [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base offset = 0
+//  [62,64) layout type (1 = SWIZZLE_128B)
+// K-major operand: rows of 128 B (64 bf16 of K), SBO = 1 KiB between 8-row groups, and a
+// step of 16 K elements advances the start address by 32 B inside the swizzle row.
+// MN-major operand: rows of 128 B hold 64 MN elements, SBO = 1 KiB between 8-row (K) groups,
+// LBO = distance between consecutive 64-wide MN chunks.
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
                                                          uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Instruction descriptor (cute::UMMA::InstrDescriptor bit layout), fp32 accum.
-//  fmt: kind::f16 -> 0 = F16, 1 = BF16 ; kind::f8f6f4 -> 0 = E4M3, 1 = E5M2
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t a_fmt, uint32_t b_fmt, bool a_mn_major,
-                                                  bool b_mn_major, uint32_t m, uint32_t n) {
-  return (1u << 4) | (a_fmt << 7) | (b_fmt << 10) | ((a_mn_major ? 1u : 0u) << 15) |
-         ((b_mn_major ? 1u : 0u) << 16) | ((n >> 3) << 17) | ((m >> 4) << 24);
+// Moves registers between warpgroups (every warp of the warpgroup executes it): the TMA
+// producer warpgroup gives registers up so the MMA warpgroups can hold their accumulators.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+
+// Named barrier over `count` threads (ids 1..15; 0 is __syncthreads).
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // -------------------------------------------------- global / peer memory ----

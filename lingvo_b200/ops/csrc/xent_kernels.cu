@@ -1,6 +1,6 @@
 // Softmax cross-entropy statistics / gradient over bf16 logits rows.
 //
-// The LM head computes logits = x . W^T with the tcgen05 GEMM (bf16 out) and
+// The LM head computes logits = x . W^T with the wgmma GEMM (bf16 out) and
 // never materialises fp32 [T, V] tensors (SURVEY K16):
 //   xent_stats : per row  lse, logit[label], sum(logits), argmax      (1 read)
 //   xent_bwd   : dlogits = p*a - b - onehot*c  written IN PLACE (bf16) where

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM front-end: `gemm`, and autograd-aware `linear` / `grouped_linear`.
+"""wgmma GEMM front-end: `gemm`, and autograd-aware `linear` / `grouped_linear`.
 
 Weights follow the reference's `[in, out]` convention (`x @ w`, SURVEY K3/K5:
 `EAM,EMH->EAH`, `BLM,MH->BLH`). The three GEMMs of a linear layer map onto the
@@ -125,7 +125,7 @@ class _LinearFn(torch.autograd.Function):
 
 
 def linear(x, w, bias=None, act=None, residual=None):
-  """x[..., K] @ w[K, N] (+bias, act | +residual) on the tcgen05 path (bf16).
+  """x[..., K] @ w[K, N] (+bias, act | +residual) on the wgmma path (bf16).
 
   `residual` (same shape as the output) is added in the GEMM epilogue — the
   sub-layer's `x + f(x)` costs no extra pass."""
@@ -213,7 +213,7 @@ class _FfnReluFn(torch.autograd.Function):
 
 
 def ffn_relu(x, wi, wo, residual=None):
-  """x[..., M] → relu(x·wi[M,H])·wo[H,M]; 4 tcgen05 GEMMs fwd+bwd, no
+  """x[..., M] → relu(x·wi[M,H])·wo[H,M]; 4 wgmma GEMMs fwd+bwd, no
   elementwise passes (bias-free FFN as in the GShard dense layers)."""
   lead = x.shape[:-1]
   x2 = x.reshape(-1, x.shape[-1])

@@ -1,4 +1,4 @@
-"""Front-end of the fused sm_100a MoE kernels (csrc/moe_kernels.cu) with their fp32 oracles.
+"""Front-end of the fused sm_90a MoE kernels (csrc/moe_kernels.cu) with their fp32 oracles.
 
 Buffer convention of the expert exchange (shared with `parallel/symm.py:MoeExchange`):
 tokens are `[T = G_l·S, M]` (G_l local groups of S tokens); every token has two expert

@@ -1,4 +1,4 @@
-"""Fused LM-head softmax cross-entropy (csrc/xent_kernels.cu + tcgen05 GEMM).
+"""Fused LM-head softmax cross-entropy (csrc/xent_kernels.cu + wgmma GEMM).
 
 `lm_head_xent(x, w, labels, label_smoothing, z_loss)` computes, per token,
 the hard-label xent, the label-smoothed xent, the z-loss increment and the

@@ -12,7 +12,7 @@ bit-for-bit up to reduction order.
 
 `AllGatherSeq` / `ReduceScatterSeq` are autograd functions (each is the other's backward),
 so any attention implementation can sit between them; `Attention()` wires the common case
-through `torch.nn.functional.scaled_dot_product_attention` (cuDNN flash on B200).
+through `torch.nn.functional.scaled_dot_product_attention` (cuDNN flash on H100).
 """
 
 from __future__ import annotations

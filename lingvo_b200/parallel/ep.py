@@ -6,7 +6,7 @@ XLA all-to-all (`gshard_layers.py:3072-3161`), TPU-only. Here it is explicit:
 * `mode='nccl'`  — stock baseline: local index-dispatch into `[E, G_l·C, M]`,
   `all_to_all_single`, grouped expert GEMMs, `all_to_all_single`, local
   index-combine.
-* `mode='fused'` — the B200 path (`ops/moe.py` + `parallel/symm.py`): the
+* `mode='fused'` — the H100 path (`ops/moe.py` + `parallel/symm.py`): the
   dispatch kernel writes every routed token row **directly into the owning
   rank's expert buffer over NVLink** (peer stores into symmetric memory), the
   second expert GEMM's epilogue stores each output row straight back into the

@@ -1,7 +1,7 @@
 """Pipeline-parallel engine: GPipe schedule over ranks with overlapped P2P links.
 
 One rank per stage (one process per GPU). Activations move forward and gradients move
-backward as `torch.distributed` point-to-point transfers — NCCL over NVLink on B200
+backward as `torch.distributed` point-to-point transfers — NCCL over NVLink on H100
 (SURVEY K14; reference `lingvo/core/gpipe.py:421-600` + `recurrent.py:1142-1400`
 Send/Recv links), gloo in the CPU tests.
 

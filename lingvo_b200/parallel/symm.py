@@ -2,7 +2,7 @@
 
 `SymmArena` — one `cudaMalloc` slab per rank whose CUDA-IPC handle is
 exchanged once; every rank maps every peer's slab, so kernels can `st`/`ld`
-straight into peers over NVLink 5 / NVSwitch (uniform any-to-any bandwidth ⇒
+straight into peers over NVLink 4 / NVSwitch (uniform any-to-any bandwidth ⇒
 flat one-hop algorithms). Buffers are bump-allocated at identical offsets on
 all ranks.
 
@@ -11,8 +11,8 @@ all ranks.
   forward   gate+dispatch kernel  : top-2 gate, slot scan, **peer stores** of
                                     every (expert, group, slot) row
             signal / wait flags   : replaces the all-to-all's barrier
-            grouped tcgen05 GEMM  : h = relu(xe · wi)
-            grouped tcgen05 GEMM  : (h · wo) with a **row-pointer epilogue**
+            grouped wgmma GEMM  : h = relu(xe · wi)
+            grouped wgmma GEMM  : (h · wo) with a **row-pointer epilogue**
                                     that stores each output row into the
                                     *source* rank's combine buffer
             signal / wait, combine: gated 2-row gather (local)

@@ -1,4 +1,4 @@
-"""Tensor-parallel FFN with the collectives fused into the tcgen05 GEMM (SURVEY K5/K6).
+"""Tensor-parallel FFN with the collectives fused into the wgmma GEMM (SURVEY K5/K6).
 
 GShard shards the FFN weights `wi[M, H]` / `wo[H, M]` on H and keeps the
 activations between layers sharded on the model dim M (`blm_split`,

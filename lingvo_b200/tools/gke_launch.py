@@ -1,7 +1,7 @@
-r"""Kubernetes launcher for B200 node pools (ref `lingvo/tools/gke_launch.py`, which deploys a
+r"""Kubernetes launcher for H100 node pools (ref `lingvo/tools/gke_launch.py`, which deploys a
 TPU trainer job, GPU decoder jobs and TensorBoard on GKE from one command line).
 
-Same workflow, B200 shape:
+Same workflow, H100 shape:
 
   * **trainer** — an Indexed `Job` with one pod per node, every pod requesting all the node's
     GPUs (`nvidia.com/gpu: 8`) and running `torchrun --nnodes=N --nproc-per-node=8 -m

@@ -8,8 +8,8 @@ this framework adds what a CUDA program needs:
 * `DeviceTimer` — CUDA-event timing of a region on the launching stream, synchronised on
   both sides, max over ranks (the contract `bench.py` follows).
 * `Roofline` — per-op time bound `max(flops / peak_flops, bytes / peak_bw)` against the
-  MEASURED peaks in `MEASURED_PEAKS.json` (driver-written; falls back to the B200 profiling
-  recipe's nominal numbers), with ready-made cost models of the fused paths.
+  measured peaks in `MEASURED_PEAKS.json` when that file exists (otherwise derated H100 SXM
+  data-sheet numbers), with ready-made cost models of the fused paths.
 """
 
 from __future__ import annotations
@@ -91,8 +91,9 @@ class DeviceTimer:
     return False
 
 
-# Nominal B200 numbers from the profiling recipe, used when no measurement file exists.
-_FALLBACK = {'hbm_gbs': 7700.0 * 0.92, 'bf16_tflops': 2250.0 * 0.75}
+# H100 SXM data sheet (3.35 TB/s HBM3, 989 dense BF16 TFLOP/s at 700 W), derated; used when
+# no measurement file exists.
+_FALLBACK = {'hbm_gbs': 3350.0 * 0.92, 'bf16_tflops': 989.0 * 0.75}
 
 
 def MeasuredPeaks(path: Optional[str] = None) -> Dict[str, float]:
@@ -105,7 +106,7 @@ def MeasuredPeaks(path: Optional[str] = None) -> Dict[str, float]:
             'bf16_tflops': float(d.get('bf16_tflops_sustained') or d['bf16_tflops']),
             'source': path}
   except (OSError, KeyError, ValueError):
-    return dict(_FALLBACK, source='fallback (B200_PROFILING.md nominal × derate)')
+    return dict(_FALLBACK, source='fallback (H100 SXM data sheet × derate)')
 
 
 class Roofline:

@@ -3,7 +3,7 @@
     python pip_package/build_pip_pkg.py [--out dist] [--skip-native] [--plat manylinux_2_34_x86_64]
 
 Steps: (1) compile the native extensions in-tree (`__graft_entry__.build()`: nvcc for
-sm_100a → `_C.so`, g++ → `_H.so`); (2) stage the package + the built `.so` files;
+sm_90a → `_C.so`, g++ → `_H.so`); (2) stage the package + the built `.so` files;
 (3) write the wheel by hand (a wheel is a zip with `WHEEL` / `METADATA` / `RECORD`), tagged
 for this interpreter and platform because it carries compiled code. No network and no
 `build` / `wheel` front-end is needed, which is what the offline image requires.
@@ -55,7 +55,7 @@ def BuildWheel(out_dir, skip_native=False, plat=None):
     for full, arc in sorted(_Files(skip_native)):
       with open(full, 'rb') as f:
         Add(arc, f.read())
-    meta = ('Metadata-Version: 2.1\nName: %s\nVersion: %s\nSummary: B200-native (sm_100a) '
+    meta = ('Metadata-Version: 2.1\nName: %s\nVersion: %s\nSummary: H100-native (sm_90a) '
             'sequence-modelling framework with the capabilities of Lingvo\n'
             'Requires-Python: >=3.10\nRequires-Dist: torch>=2.4\nRequires-Dist: numpy\n'
             'Requires-Dist: pyyaml\nRequires-Dist: absl-py\n' % (NAME, VERSION))

@@ -1,4 +1,4 @@
-"""Packaging (ref `pip_package/`): `pip install .` builds the sm_100a kernel extension and
+"""Packaging (ref `pip_package/`): `pip install .` builds the sm_90a kernel extension and
 the host runtime in-tree through `lingvo_b200.ops.build`, then installs the package."""
 
 import os
@@ -22,7 +22,7 @@ class BuildWithExtensions(build_py):
 setup(
     name='lingvo_b200',
     version='0.2.0',
-    description='B200-native (sm_100a) sequence-modelling framework with the capabilities of Lingvo',
+    description='H100-native (sm_90a) sequence-modelling framework with the capabilities of Lingvo',
     packages=find_packages(include=['lingvo_b200', 'lingvo_b200.*']),
     package_data={'lingvo_b200.ops': ['*.so', 'csrc/*', 'csrc_host/*']},
     python_requires='>=3.10',

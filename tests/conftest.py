@@ -7,7 +7,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def pytest_configure(config):
-  config.addinivalue_line('markers', 'gpu: test needs a CUDA (B200) device')
+  config.addinivalue_line('markers', 'gpu: test needs a CUDA (H100) device')
   config.addinivalue_line('markers', 'slow: long-running test')
 
 

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM numerics vs a plain PyTorch fp32 reference."""
+"""wgmma GEMM numerics vs a plain PyTorch fp32 reference."""
 import pytest
 import torch
 

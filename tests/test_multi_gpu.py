@@ -33,7 +33,7 @@ def test_fused_ep_dp_matches_nccl_baseline():
 
 
 def test_tensor_parallel_ffn_matches_oracle():
-  """TP FFN with collectives fused into the tcgen05 GEMM vs fp32 single-device oracle."""
+  """TP FFN with collectives fused into the wgmma GEMM vs fp32 single-device oracle."""
   _NeedGpus(2)
   rc, out = _Run('tools/tp_check.py', 2, 29622, '2048', '1024', '2048')
   assert rc == 0 and 'TP_OK' in out, out[-3000:]
@@ -49,7 +49,7 @@ def test_product_trainer_two_gpus_identical_replicas_resume_and_gradients():
 
 def test_tensor_parallel_model_matches_single_gpu():
   """DenseBuilder UniTransformer with heads / FFN hidden sharded over 2 GPUs (NCCL f/g +
-  local tcgen05 GEMMs): loss, gathered gradients and 8 Adam steps ≈ the unsharded model."""
+  local wgmma GEMMs): loss, gathered gradients and 8 Adam steps ≈ the unsharded model."""
   _NeedGpus(2)
   rc, out = _Run('tools/tp_model_check.py', 2, 29624)
   assert rc == 0 and 'TP_MODEL_OK' in out, out[-4000:]

@@ -6,7 +6,7 @@ Run under torchrun on N GPUs. For every size: time = CUDA events around
 `iters`. Traffic model of a two-shot all-reduce of S bytes per rank over W ranks: every rank
 *reads* (W−1)/W·S from its peers (reduce-scatter phase) and *writes* (W−1)/W·S to them
 (all-gather phase), so per-GPU NVLink traffic is (W−1)/W·S in each direction; the roofline is
-that volume over the 900 GB/s per-direction NVLink 5 rate. Also reports the capped-grid
+that volume over the 450 GB/s per-direction NVLink-4 rate of an H100 SXM. Also reports the capped-grid
 variant used while overlapping with backward (`max_blocks=48`) and `dist.all_reduce`.
 Writes gpurun_out/allreduce_bench_n<W>.json.
 """
@@ -18,7 +18,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import torch.distributed as dist
 
-NVLINK_GBS = 900.0
+NVLINK_GBS = 450.0
 
 
 def Time(fn, iters=20, warmup=5):

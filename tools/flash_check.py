@@ -1,4 +1,4 @@
-"""GPU check + timing of the tcgen05 flash attention (csrc/flash_attn.cu).
+"""GPU check + timing of the wgmma flash attention (csrc/flash_attn.cu).
 
 Numerics against the fp32 oracle for forward, dQ/dK/dV and the bias-table gradient
 (several geometries: packed segments, padding, causal / bidirectional, with / without the

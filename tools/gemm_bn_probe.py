@@ -1,4 +1,4 @@
-"""Tile-N A/B of the tcgen05 GEMM on the flagship model's shapes (run on a GPU box; each
+"""Tile-N A/B of the wgmma GEMM on the flagship model's shapes (run on a GPU box; each
 setting needs its own process because the override is read once):
 
   for bn in 256 128; do LINGVO_B200_GEMM_BN=$bn python tools/gemm_bn_probe.py; done

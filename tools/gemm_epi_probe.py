@@ -1,4 +1,4 @@
-"""Times the tcgen05 GEMM epilogue variants on FFN shapes (1 GPU)."""
+"""Times the wgmma GEMM epilogue variants on FFN shapes (1 GPU)."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""Times the tcgen05 GEMM vs cuBLAS (torch.matmul) with CUDA events."""
+"""Times the wgmma GEMM vs cuBLAS (torch.matmul) with CUDA events."""
 import json
 import sys
 import torch

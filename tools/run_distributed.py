@@ -2,7 +2,7 @@
 """Local multi-process launcher (ref `docker/run_distributed.py`: a docker fleet of
 `worker×3, controller, trainer_client` (sync) or `trainer×3, ps×2, controller` (async)).
 
-On B200 the topology is one process per GPU: a *trainer* job of N ranks under
+On H100 the topology is one process per GPU: a *trainer* job of N ranks under
 `torch.distributed.run`, plus optional *evaler* / *decoder* side jobs that poll the same
 log dir (they need no rendezvous with the trainer).
 

@@ -1,6 +1,6 @@
 """Multi-GPU check of the fused tensor-parallel FFN (run under torchrun).
 
-Compares `parallel.tp.TpFfn` (collectives inside the tcgen05 GEMM) against an
+Compares `parallel.tp.TpFfn` (collectives inside the wgmma GEMM) against an
 fp32 single-device oracle for forward and all gradients, then times it against
 the NCCL all_gather + cuBLAS + reduce_scatter baseline.
 """

@@ -3,7 +3,7 @@
 Builds the GShard dense UniTransformer twice in every process with identical (name-seeded)
 logical weights:
   * TP:     `device_mesh_shape=[1, N]` → attention heads and FFN hidden dim sharded N ways,
-            NCCL all-reduce at the two region boundaries, local tcgen05 GEMMs;
+            NCCL all-reduce at the two region boundaries, local wgmma GEMMs;
   * oracle: the same model unsharded on this GPU.
 Checks, in bf16 compute with fp32 masters: loss, per-variable gradients (shards gathered),
 and 5 Adafactor/Adam steps; then reports ms/step of both for the strong-scaling record.
