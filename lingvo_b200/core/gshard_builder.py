@@ -553,6 +553,36 @@ def _SelfAttentionExtendStep(layer, theta, x, cache, t):
   if b.use_rotary_position_emb or (layer.params.multi_dconv_head and b.mdha_rope):
     pos = tt.reshape(1, 1).expand(bsz, 1)
     q, k = _Rope(q, pos, b.rope_emb_max_timescale), _Rope(k, pos, b.rope_emb_max_timescale)
+  if b.atten_logit_cap:
+    o = _CappedDecodeAttention(layer, theta, q, k, v, cache, tt)
+  else:
+    # Fused cache append + attention over the live keys (our split-KV kernel on the GPU).
+    from lingvo_b200.ops import attention as attention_ops
+    rel = None
+    if layer.params.relative_bias:
+      bucket = RelativePositionBucket(     # table[:, i] for key − query = T − 1 − i
+          torch.arange(tmax - 1, -tmax, -1, device=dev), b.relative_attention_num_buckets,
+          b.relative_attention_max_distance,
+          bidirectional=b.decoder_bidirectional_relative_attention)
+      rel = theta.wrb.float()[:, bucket.long()]
+    o = attention_ops.decode_attention(q, k, v, cache.k, cache.v, tt, rel)
+    o = o.reshape(bsz, 1, h * d)
+  out = torch.matmul(o, theta.wo.to(xd))
+  if layer._tp is not None:   # pylint: disable=protected-access
+    from lingvo_b200.parallel import tp_layers   # pylint: disable=g-import-not-at-top
+    out = tp_layers.ReduceFromTensorParallel(out, layer._tp)   # pylint: disable=protected-access
+  return out
+
+
+def _CappedDecodeAttention(layer, theta, q, k, v, cache, tt):
+  """Decode-step attention of a layer with `atten_logit_cap`: one-hot cache write, fp32 logits
+  over every cached key, the cap applied to q·k + bias − 1e9·future. Returns `[B,1,H·D]`."""
+  b = layer.bp
+  bsz, _, h, d = q.shape
+  hk = k.shape[2]
+  xd = q.dtype
+  tmax = cache.k.shape[1]
+  dev = q.device
   onehot = (torch.arange(tmax, device=dev) == tt).to(xd).reshape(1, tmax, 1, 1)
   cache.k.mul_(1 - onehot).add_(k * onehot)
   cache.v.mul_(1 - onehot).add_(v * onehot)
@@ -571,11 +601,7 @@ def _SelfAttentionExtendStep(layer, theta, x, cache, t):
     logits = b.atten_logit_cap * torch.tanh(logits / b.atten_logit_cap)
   probs = torch.softmax(logits, -1)
   o = torch.einsum('bhqk,bkhd->bqhd', probs, vv.float()).to(xd).reshape(bsz, 1, h * d)
-  out = torch.matmul(o, theta.wo.to(xd))
-  if layer._tp is not None:   # pylint: disable=protected-access
-    from lingvo_b200.parallel import tp_layers   # pylint: disable=g-import-not-at-top
-    out = tp_layers.ReduceFromTensorParallel(out, layer._tp)   # pylint: disable=protected-access
-  return out
+  return o
 
 
 def _Rope(x, pos, max_timescale):

@@ -257,3 +257,68 @@ def flash_attention(q, k, v, rel=None, seg=None, pos=None, scale=1.0, causal=Fal
     pos = pos.to(torch.int32).contiguous()
   return _FlashAttnFn.apply(_View(q), _View(k), _View(v), rel, seg, pos, float(scale),
                             bool(causal))
+
+
+# ------------------------------------------------------- incremental decoding ----
+def decode_attention_ref(q, k_new, v_new, k_cache, v_cache, t, rel=None, scale=1.0):
+  """fp32 oracle and CPU path of `decode_attention`: one-hot write of row t into the caches,
+  fp32 logits over all T keys, −1e9 on the keys after t. Grouped / multi-query KV heads are
+  expanded with `_ExpandKv`."""
+  bsz, _, h, _ = q.shape
+  tmax = k_cache.shape[1]
+  dev = q.device
+  tt = torch.as_tensor(t, device=dev).reshape(())
+  onehot = (torch.arange(tmax, device=dev) == tt).to(k_cache.dtype).reshape(1, tmax, 1, 1)
+  k_cache.mul_(1 - onehot).add_(k_new * onehot)
+  v_cache.mul_(1 - onehot).add_(v_new * onehot)
+  kk, vv = _ExpandKv(k_cache, h), _ExpandKv(v_cache, h)
+  logits = torch.einsum('bqhd,bkhd->bhqk', q.float(), kk.float())      # [B,H,1,T]
+  if scale != 1.0:
+    logits = logits * scale
+  key_pos = torch.arange(tmax, device=dev)
+  if rel is not None:
+    idx = (tt - key_pos + tmax - 1).clamp(0, 2 * tmax - 2)
+    logits = logits + rel.float()[:, idx].reshape(1, h, 1, tmax)
+  logits = logits + ((key_pos > tt).float() * -1e9).reshape(1, 1, 1, tmax)
+  probs = torch.softmax(logits, -1)
+  return torch.einsum('bhqk,bkhd->bqhd', probs, vv.float()).to(q.dtype)
+
+
+def decode_attention_supported(q, k_cache):
+  from lingvo_b200 import ops
+  mod = ops.native(required=False) if q.is_cuda else None
+  return (mod is not None and hasattr(mod, '_has_decode_attn') and
+          ops.use_cuda_kernels(q, k_cache) and q.dtype == torch.bfloat16 and
+          k_cache.dtype == torch.bfloat16 and q.dim() == 4 and k_cache.dim() == 4 and
+          q.shape[-1] == 128 and k_cache.shape[-1] == 128 and
+          q.shape[2] % k_cache.shape[2] == 0 and k_cache.is_contiguous())
+
+
+def decode_attention(q, k_new, v_new, k_cache, v_cache, t, rel=None, scale=1.0):
+  """One decode step of self-attention for a single query token per sequence.
+
+  q `[B,1,H,D]`, k_new / v_new `[B,1,Hk,D]` (Hk divides H; query head h reads KV head
+  h // (H/Hk)), caches `[B,T,Hk,D]` updated in place at row t, `t` a Python int or 0-dim
+  integer tensor, `rel` an optional fp32 `[H, 2T-1]` table indexed by t − j + T − 1 (clamped
+  to the table). Keys j ≤ t are visible; for t outside [0, T) no row is written and all keys
+  are. Returns `[B,1,H,D]`.
+
+  On the GPU (bf16, D = 128) this is our split-KV kernel (csrc/decode_attn.cu): it reads
+  only the live rows of the cache and its launch shape does not depend on t, so a step with
+  `t` as a device scalar can be captured in a CUDA graph.
+  """
+  if not decode_attention_supported(q, k_cache):
+    return decode_attention_ref(q, k_new, v_new, k_cache, v_cache, t, rel, scale)
+  from lingvo_b200 import ops
+  b, _, h, d = q.shape
+  hk = k_cache.shape[2]
+  tt = torch.as_tensor(t, device=q.device)
+  if tt.dtype not in (torch.int32, torch.int64):
+    tt = tt.long()
+  if rel is not None:
+    rel = rel.float().contiguous()
+  out = ops.native().decode_attn_fwd(
+      q.reshape(b, h, d).contiguous(), k_new.reshape(b, hk, d).contiguous(),
+      v_new.reshape(b, hk, d).contiguous(), k_cache, v_cache, tt.reshape(()), rel,
+      float(scale))
+  return out.reshape(b, 1, h, d)
