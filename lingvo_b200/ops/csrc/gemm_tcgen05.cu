@@ -11,14 +11,25 @@
 // * two consumer warpgroups each own 64 rows of the 128 x BN tile and issue
 //   wgmma.m64nBNk16 (fp32 accumulators in registers), keeping one k-block of
 //   MMAs in flight while the next stage is awaited;
+// * the kernel is persistent: min(tiles, SMs) CTAs walk the output tiles of all
+//   groups in a fixed order (bands of kGroupM M-tiles, for L2 reuse), and the
+//   producer runs ahead across tile boundaries, so the ring refills for the next
+//   tile while the consumers run this tile's epilogue;
 // * the fused epilogue (bias, activation, relu-gradient mask / residual add,
-//   per-row scale, accumulate) runs on the accumulator registers and stores
-//   straight to global memory.  The store target of every output row can be
-//   redirected through a row-pointer table, which is how the MoE combine
-//   (expert GEMM -> NVLink peer store) is fused.
+//   per-row scale, accumulate) stages the accumulators through shared memory,
+//   64 columns at a time, and then works on 8 adjacent columns of a row per
+//   thread, so every global load and store is a 16-byte row-contiguous vector.
+//   The store target of every output row can be redirected through a
+//   row-pointer table, which is how the MoE combine (expert GEMM -> NVLink peer
+//   store) is fused.
 //
-// Grid: one CTA per output tile, 288 threads:
-//   warps 0..7 = two consumer warpgroups, warp 8 = TMA producer.
+// Every output tile is computed by one CTA with the same k-block order and wgmma
+// shape as a one-tile-per-CTA launch, so results do not depend on the grid size.
+//
+// 384 threads: warps 0..7 = two consumer warpgroups, warps 8..11 = producer warpgroup
+// (one thread issues TMA). The producer gives its registers to the consumers with
+// setmaxnreg: the 128 fp32 accumulators plus the epilogue do not fit in the 168 registers
+// per thread that a 384-thread CTA gets by default.
 
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -36,7 +47,9 @@ constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;   // 64 bf16 = 128 bytes = one swizzle row
 constexpr int kMmaK = 16;
 constexpr int kNumConsumers = 256;                 // two warpgroups x 64 rows
-constexpr int kNumThreads = kNumConsumers + 32;    // + one TMA producer warp
+constexpr int kNumThreads = kNumConsumers + 128;   // + the TMA producer warpgroup
+constexpr int kEpiCols = 64;  // columns per epilogue staging slice
+constexpr int kGroupM = 8;    // M-tiles per rasterisation band
 
 enum Act : int { kActNone = 0, kActRelu = 1, kActGelu = 2, kActSilu = 3, kActGeluTanh = 4,
                  kActSquaredRelu = 5 };
@@ -82,50 +95,58 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   }
 }
 
-struct EpiRow {
-  void* c_row;
-  long long row_off;
-  const float* bias;
-  float rscale;
-};
-
-// One pair of adjacent output columns (col, col + 1) of one row: bias / pre-act tap /
-// activation / aux (ReLU-mask or residual add) / row scale / convert / store.
+// Eight adjacent output columns of one row, read row-contiguously from the staging buffer:
+// bias / pre-act tap / activation / aux (ReLU-mask or residual add) / row scale / convert /
+// store. `off` is the element offset of (row, col) in the C-shaped aux / pre_act tensors,
+// `dst` the destination of (row, col); all of them are 16-byte aligned.
 template <typename OutT>
-__device__ __forceinline__ void epilogue_pair(const GemmParams& p, const EpiRow& er, float f0,
-                                              float f1, int col) {
-  if (er.bias != nullptr) {
-    const float2 b = __ldg(reinterpret_cast<const float2*>(er.bias + col));
-    f0 += b.x; f1 += b.y;
+__device__ __forceinline__ void epilogue_vec8(const GemmParams& p, float (&v)[8], OutT* dst,
+                                              long long off, const float* bias, float rscale) {
+  if (bias != nullptr) {
+    const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias));
+    const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias) + 1);
+    v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w;
+    v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;
   }
   if (p.pre_act != nullptr) {
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.pre_act) + er.row_off + col) =
-        pack_bf16x2(f0, f1);
+    const int4 o = make_int4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]),
+                             pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+    *reinterpret_cast<int4*>(reinterpret_cast<__nv_bfloat16*>(p.pre_act) + off) = o;
   }
-  f0 = apply_act(f0, p.act);
-  f1 = apply_act(f1, p.act);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) v[j] = apply_act(v[j], p.act);
   if (p.aux_mode != kAuxNone) {
-    const float2 t = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.aux + er.row_off + col));
-    if (p.aux_mode == kAuxReluMask) {
-      f0 = t.x > 0.f ? f0 : 0.f;
-      f1 = t.y > 0.f ? f1 : 0.f;
-    } else {
-      f0 += t.x;
-      f1 += t.y;
+    const int4 raw = *reinterpret_cast<const int4*>(p.aux + off);
+    const uint32_t w[4] = {static_cast<uint32_t>(raw.x), static_cast<uint32_t>(raw.y),
+                           static_cast<uint32_t>(raw.z), static_cast<uint32_t>(raw.w)};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 t = unpack_bf16x2(w[j]);
+      if (p.aux_mode == kAuxReluMask) {
+        v[2 * j] = t.x > 0.f ? v[2 * j] : 0.f;
+        v[2 * j + 1] = t.y > 0.f ? v[2 * j + 1] : 0.f;
+      } else {
+        v[2 * j] += t.x;
+        v[2 * j + 1] += t.y;
+      }
     }
   }
-  f0 *= er.rscale;
-  f1 *= er.rscale;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) v[j] *= rscale;
   if constexpr (sizeof(OutT) == 2) {
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(er.c_row) + col) = pack_bf16x2(f0, f1);
+    *reinterpret_cast<int4*>(dst) = make_int4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]),
+                                              pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
   } else {
-    float2* out = reinterpret_cast<float2*>(reinterpret_cast<float*>(er.c_row) + col);
-    float2 o = make_float2(f0, f1);
+    float4* out = reinterpret_cast<float4*>(dst);
+    float4 o0 = make_float4(v[0], v[1], v[2], v[3]);
+    float4 o1 = make_float4(v[4], v[5], v[6], v[7]);
     if (p.accumulate) {
-      const float2 old = *out;
-      o.x += old.x; o.y += old.y;
+      const float4 a0 = out[0], a1 = out[1];
+      o0.x += a0.x; o0.y += a0.y; o0.z += a0.z; o0.w += a0.w;
+      o1.x += a1.x; o1.y += a1.y; o1.z += a1.z; o1.w += a1.w;
     }
-    *out = o;
+    out[0] = o0;
+    out[1] = o1;
   }
 }
 
@@ -135,20 +156,57 @@ __device__ __forceinline__ void wgmma_bn(float (&acc)[BN / 2], uint64_t adesc, u
   else wgmma_m64n128k16<kAK ? 0 : 1, kBK ? 0 : 1>(acc, adesc, bdesc, 1);
 }
 
+template <int BN>
+struct TileShape {
+  static constexpr int kStages = (BN == 256) ? 4 : 6;
+  static constexpr uint32_t kABytes = kBlockM * kBlockK * 2;   // 16 KiB
+  static constexpr uint32_t kBBytes = BN * kBlockK * 2;        // 32 KiB (BN=256)
+  static constexpr uint32_t kStageBytes = kABytes + kBBytes;
+  static constexpr uint32_t kRingBytes = kStages * kStageBytes;
+  // fp32 epilogue staging: 64 rows x 64 columns per consumer warpgroup.
+  static constexpr uint32_t kStagingBytes = 2 * 64 * kEpiCols * 4;
+  static constexpr size_t kSmemBytes = kRingBytes + kStagingBytes + 2 * kStages * 8 + 1024;
+};
+
+// Tiles are numbered group by group. Inside a group they go in bands of kGroupM M-tiles,
+// M-fastest inside a band: the CTAs of one wave then share a few A panels and B panels in L2.
+struct TileCoord {
+  int g, m_blk, n_blk;
+};
+__device__ __forceinline__ TileCoord tile_coord(int tile, int tiles_m, int tiles_n) {
+  const int per_group = tiles_m * tiles_n;
+  TileCoord t;
+  t.g = tile / per_group;
+  const int r = tile - t.g * per_group;
+  const int band = r / (kGroupM * tiles_n);
+  const int first_m = band * kGroupM;
+  const int rows = min(kGroupM, tiles_m - first_m);
+  const int in_band = r - band * kGroupM * tiles_n;
+  t.n_blk = in_band / rows;
+  t.m_blk = first_m + (in_band - t.n_blk * rows);
+  return t;
+}
+
+// Byte offset of the 16-byte unit u (of 16) in row r of a warpgroup's staging buffer. The
+// XOR spreads both the fragment writes (4 rows x 2 units per half-warp) and the
+// row-contiguous reads (8 units of one row per quarter-warp) over all 32 banks.
+__device__ __forceinline__ uint32_t staging_off(int r, int u) {
+  return static_cast<uint32_t>(r * (kEpiCols / 4) + (u ^ ((r & 7) << 1))) * 16;
+}
+
 template <int BN, bool kAK, bool kBK, typename OutT>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
                   const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
-  constexpr int kStages = (BN == 256) ? 4 : 6;
-  constexpr uint32_t kABytes = kBlockM * kBlockK * 2;   // 16 KiB
-  constexpr uint32_t kBBytes = BN * kBlockK * 2;        // 32 KiB (BN=256)
-  constexpr uint32_t kStageBytes = kABytes + kBBytes;
+  using TS = TileShape<BN>;
+  constexpr int kStages = TS::kStages;
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024B alignment for SWIZZLE_128B atoms.
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
+  uint8_t* staging = smem + TS::kRingBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + TS::kStagingBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
 
@@ -156,12 +214,8 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
   const int lane = threadIdx.x & 31;
 
   const int tiles_m = (p.M + kBlockM - 1) / kBlockM;
-  const int tiles_per_group = tiles_m * ((p.N + BN - 1) / BN);
-  const int g = blockIdx.x / tiles_per_group;
-  const int r = blockIdx.x - g * tiles_per_group;
-  const int n_blk = r / tiles_m;
-  const int m_blk = r - n_blk * tiles_m;
-  const int m0 = m_blk * kBlockM, n0 = n_blk * BN;
+  const int tiles_n = (p.N + BN - 1) / BN;
+  const int num_tiles = p.G * tiles_m * tiles_n;
   const int num_k_blocks = (p.K + kBlockK - 1) / kBlockK;
 
   if (threadIdx.x == kNumConsumers) {
@@ -175,32 +229,41 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
   }
   __syncthreads();
 
-  if (warp_idx == kNumConsumers / 32) {
+  // The ring position (stage, phase) runs on across tiles in both roles, so the producer
+  // fills the stages for the next tile while the consumers run this tile's epilogue.
+  if (warp_idx >= kNumConsumers / 32) {
     // ============================ TMA producer ============================
-    if (lane == 0) {
-      for (int kb = 0; kb < num_k_blocks; ++kb) {
-        const int stage = kb % kStages;
-        mbar_wait(smem_u32(&empty_bar[stage]), ((kb / kStages) & 1) ^ 1);
-        const uint32_t fb = smem_u32(&full_bar[stage]);
-        mbar_arrive_expect_tx(fb, kStageBytes);
-        const uint32_t sa = smem_u32(smem + stage * kStageBytes);
-        const uint32_t sb = sa + kABytes;
-        const int k0 = kb * kBlockK;
-        const int amap = k0 / p.a_k_per_map;
-        const int ka = k0 - amap * p.a_k_per_map;
-        if constexpr (kAK) {
-          tma_load_3d(sa, &tmaps_a.m[amap], fb, ka, m0, g);
-        } else {
+    setmaxnreg_dec<40>();
+    if (warp_idx == kNumConsumers / 32 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const TileCoord tc = tile_coord(tile, tiles_m, tiles_n);
+        const int m0 = tc.m_blk * kBlockM, n0 = tc.n_blk * BN, g = tc.g;
+        for (int kb = 0; kb < num_k_blocks; ++kb) {
+          mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
+          const uint32_t fb = smem_u32(&full_bar[stage]);
+          mbar_arrive_expect_tx(fb, TS::kStageBytes);
+          const uint32_t sa = smem_u32(smem + stage * TS::kStageBytes);
+          const uint32_t sb = sa + TS::kABytes;
+          const int k0 = kb * kBlockK;
+          const int amap = k0 / p.a_k_per_map;
+          const int ka = k0 - amap * p.a_k_per_map;
+          if constexpr (kAK) {
+            tma_load_3d(sa, &tmaps_a.m[amap], fb, ka, m0, g);
+          } else {
 #pragma unroll
-          for (int i = 0; i < kBlockM / 64; ++i)
-            tma_load_3d(sa + i * (64 * kBlockK * 2), &tmaps_a.m[amap], fb, m0 + 64 * i, ka, g);
-        }
-        if constexpr (kBK) {
-          tma_load_3d(sb, &tmap_b, fb, k0, n0, g);
-        } else {
+            for (int i = 0; i < kBlockM / 64; ++i)
+              tma_load_3d(sa + i * (64 * kBlockK * 2), &tmaps_a.m[amap], fb, m0 + 64 * i, ka, g);
+          }
+          if constexpr (kBK) {
+            tma_load_3d(sb, &tmap_b, fb, k0, n0, g);
+          } else {
 #pragma unroll
-          for (int i = 0; i < BN / 64; ++i)
-            tma_load_3d(sb + i * (64 * kBlockK * 2), &tmap_b, fb, n0 + 64 * i, k0, g);
+            for (int i = 0; i < BN / 64; ++i)
+              tma_load_3d(sb + i * (64 * kBlockK * 2), &tmap_b, fb, n0 + 64 * i, k0, g);
+          }
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
@@ -210,60 +273,106 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
   // ============================== consumers ==============================
   // Warpgroup wg owns tile rows [64 wg, 64 wg + 64). Its A rows start 8 KiB into the
   // stage for both majors: 64 K-major rows of 128 B, or the wg-th 64-wide MN chunk.
+  setmaxnreg_inc<232>();
   const int wg = warp_idx >> 2;
-  float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  for (int kb = 0; kb < num_k_blocks; ++kb) {
-    const int stage = kb % kStages;
-    mbar_wait(smem_u32(&full_bar[stage]), (kb / kStages) & 1);
-    const uint32_t sa = smem_u32(smem + stage * kStageBytes) + wg * (64 * 128);
-    const uint32_t sb = smem_u32(smem + stage * kStageBytes) + kABytes;
-    wgmma_fence();
-#pragma unroll
-    for (int j = 0; j < kBlockK / kMmaK; ++j) {
-      // K-major: advance 32 B inside the 128 B swizzle row.
-      // MN-major: advance 16 K-rows of 128 B; 64-wide MN chunks are
-      //           64*kBlockK*2 bytes apart (LBO), 8-row groups 1 KiB (SBO).
-      const uint64_t adesc =
-          kAK ? make_smem_desc_sw128(sa + j * 32, 16, 1024)
-              : make_smem_desc_sw128(sa + j * (kMmaK * 128), 64 * kBlockK * 2, 1024);
-      const uint64_t bdesc =
-          kBK ? make_smem_desc_sw128(sb + j * 32, 16, 1024)
-              : make_smem_desc_sw128(sb + j * (kMmaK * 128), 64 * kBlockK * 2, 1024);
-      wgmma_bn<BN, kAK, kBK>(acc, adesc, bdesc);
-    }
-    wgmma_commit();
-    wgmma_wait<1>();                 // the previous k-block's MMAs have retired
-    __syncwarp();
-    if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[(kb - 1) % kStages]));
-  }
-  wgmma_wait<0>();
-  wgmma_fence_regs(acc);
+  const uint32_t stg = smem_u32(staging + wg * (64 * kEpiCols * 4));
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const TileCoord tc = tile_coord(tile, tiles_m, tiles_n);
+    const int m0 = tc.m_blk * kBlockM, n0 = tc.n_blk * BN, g = tc.g;
 
-  // ============================== epilogue ==============================
-  const int wrow = m0 + wg * 64 + (warp_idx & 3) * 16 + (lane >> 2);
-  const int cq = (lane & 3) * 2;
+    float acc[BN / 2];
 #pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int row = wrow + 8 * i;
-    if (row >= p.M) continue;
-    EpiRow er;
-    er.row_off = static_cast<long long>(g) * p.c_batch + static_cast<long long>(row) * p.ldc;
-    if (p.row_ptrs != nullptr) {
-      er.c_row = p.row_ptrs[static_cast<long long>(g) * p.M + row];
-    } else if (p.nblk_ptrs != nullptr) {
-      er.c_row = reinterpret_cast<OutT*>(p.nblk_ptrs[n_blk]) + static_cast<long long>(row) * p.ldc - n0;
-    } else {
-      er.c_row = reinterpret_cast<OutT*>(p.c) + er.row_off;
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev_stage = 0;
+    for (int kb = 0; kb < num_k_blocks; ++kb) {
+      mbar_wait(smem_u32(&full_bar[stage]), phase);
+      const uint32_t sa = smem_u32(smem + stage * TS::kStageBytes) + wg * (64 * 128);
+      const uint32_t sb = smem_u32(smem + stage * TS::kStageBytes) + TS::kABytes;
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < kBlockK / kMmaK; ++j) {
+        // K-major: advance 32 B inside the 128 B swizzle row.
+        // MN-major: advance 16 K-rows of 128 B; 64-wide MN chunks are
+        //           64*kBlockK*2 bytes apart (LBO), 8-row groups 1 KiB (SBO).
+        const uint64_t adesc =
+            kAK ? make_smem_desc_sw128(sa + j * 32, 16, 1024)
+                : make_smem_desc_sw128(sa + j * (kMmaK * 128), 64 * kBlockK * 2, 1024);
+        const uint64_t bdesc =
+            kBK ? make_smem_desc_sw128(sb + j * 32, 16, 1024)
+                : make_smem_desc_sw128(sb + j * (kMmaK * 128), 64 * kBlockK * 2, 1024);
+        wgmma_bn<BN, kAK, kBK>(acc, adesc, bdesc);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                 // the previous k-block's MMAs have retired
+      __syncwarp();
+      if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_stage]));
+      prev_stage = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
-    if (er.c_row == nullptr) continue;
-    er.rscale = p.row_scale != nullptr ? p.row_scale[static_cast<long long>(g) * p.M + row] : 1.f;
-    er.bias = p.bias ? p.bias + static_cast<long long>(g) * p.N : nullptr;
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    __syncwarp();
+    if (num_k_blocks > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_stage]));
+
+    // ============================ epilogue ============================
+    // Per 64-column slice: fragments -> staging (fp32), then each thread takes 8 adjacent
+    // columns of a row, so every global access is a 16-byte row-contiguous vector.
+    const int frow = (warp_idx & 3) * 16 + (lane >> 2);
+    const int q = threadIdx.x & 7;          // 8-column chunk of the slice
+    const int rsub = (threadIdx.x & 127) >> 3;
+    const int first = (q >> 2) & 1;        // which half of the chunk to read first (banks)
 #pragma unroll
-    for (int n = 0; n < BN / 8; ++n) {
-      const int col = n0 + n * 8 + cq;
-      if (col < p.N) epilogue_pair<OutT>(p, er, acc[4 * n + 2 * i], acc[4 * n + 2 * i + 1], col);
+    for (int s = 0; s < BN / kEpiCols; ++s) {
+      if (n0 + s * kEpiCols >= p.N) break;
+      named_bar_sync(1 + wg, 128);         // the previous slice's reads are done
+#pragma unroll
+      for (int n = 0; n < kEpiCols / 8; ++n) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int a = 4 * (s * (kEpiCols / 8) + n) + 2 * i;
+          const uint32_t addr = stg + staging_off(frow + 8 * i, 2 * n + ((lane & 3) >> 1)) +
+                                (lane & 1) * 8;
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(acc[a]),
+                       "f"(acc[a + 1]) : "memory");
+        }
+      }
+      named_bar_sync(1 + wg, 128);
+      const int col = n0 + s * kEpiCols + 8 * q;
+#pragma unroll
+      for (int pass = 0; pass < 4; ++pass) {
+        const int r = rsub + 16 * pass;
+        const int row = m0 + wg * 64 + r;
+        if (row >= p.M || col >= p.N) continue;
+        OutT* dst;
+        const long long row_off =
+            static_cast<long long>(g) * p.c_batch + static_cast<long long>(row) * p.ldc;
+        if (p.row_ptrs != nullptr) {
+          dst = reinterpret_cast<OutT*>(p.row_ptrs[static_cast<long long>(g) * p.M + row]);
+          if (dst == nullptr) continue;
+          dst += col;
+        } else if (p.nblk_ptrs != nullptr) {
+          // one destination slab per 256 output columns
+          dst = reinterpret_cast<OutT*>(p.nblk_ptrs[col >> 8]) +
+                static_cast<long long>(row) * p.ldc + (col & 255);
+        } else {
+          dst = reinterpret_cast<OutT*>(p.c) + row_off + col;
+        }
+        float4 h0, h1;
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                     : "=f"(h0.x), "=f"(h0.y), "=f"(h0.z), "=f"(h0.w)
+                     : "r"(stg + staging_off(r, 2 * q + first)) : "memory");
+        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                     : "=f"(h1.x), "=f"(h1.y), "=f"(h1.z), "=f"(h1.w)
+                     : "r"(stg + staging_off(r, 2 * q + 1 - first)) : "memory");
+        const float4 lo = first ? h1 : h0, hi = first ? h0 : h1;
+        float v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+        const float rscale =
+            p.row_scale != nullptr ? p.row_scale[static_cast<long long>(g) * p.M + row] : 1.f;
+        const float* bias = p.bias ? p.bias + static_cast<long long>(g) * p.N + col : nullptr;
+        epilogue_vec8<OutT>(p, v, dst, row_off + col, bias, rscale);
+      }
     }
   }
 }
@@ -313,9 +422,9 @@ CUtensorMap MakeMap(const void* base, int64_t inner, int64_t rows, int64_t group
 
 template <int BN, bool kAK, bool kBK, typename OutT>
 static void Launch(const TmapArray& ta, const CUtensorMap& tb, const GemmParams& p,
-                   cudaStream_t stream) {
-  constexpr int kStages = (BN == 256) ? 4 : 6;
-  constexpr size_t smem = kStages * (kBlockM * kBlockK * 2 + BN * kBlockK * 2) + 1024 + 256;
+                   int sms, cudaStream_t stream) {
+  constexpr size_t smem = TileShape<BN>::kSmemBytes;
+  static_assert(smem <= 227 * 1024, "GEMM shared memory exceeds the sm_90 limit");
   auto kern = gemm_wgmma_kernel<BN, kAK, kBK, OutT>;
   static bool configured = false;
   if (!configured) {
@@ -323,29 +432,34 @@ static void Launch(const TmapArray& ta, const CUtensorMap& tb, const GemmParams&
                                         static_cast<int>(smem)));
     configured = true;
   }
-  const int tiles = p.G * ((p.M + kBlockM - 1) / kBlockM) * ((p.N + BN - 1) / BN);
-  kern<<<tiles, kNumThreads, smem, stream>>>(ta, tb, p);
+  const int64_t tiles = static_cast<int64_t>(p.G) * ((p.M + kBlockM - 1) / kBlockM) *
+                        ((p.N + BN - 1) / BN);
+  TORCH_CHECK(tiles < (int64_t{1} << 31), "gemm_bf16: too many output tiles");
+  const int grid = static_cast<int>(std::min<int64_t>(tiles, sms));
+  kern<<<grid, kNumThreads, smem, stream>>>(ta, tb, p);
   CountLaunch();
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
 template <int BN, typename OutT>
 static void Dispatch(bool ak, bool bk, const TmapArray& ta, const CUtensorMap& tb,
-                     const GemmParams& p, cudaStream_t s) {
-  if (ak && bk) Launch<BN, true, true, OutT>(ta, tb, p, s);
-  else if (ak && !bk) Launch<BN, true, false, OutT>(ta, tb, p, s);
-  else if (!ak && bk) Launch<BN, false, true, OutT>(ta, tb, p, s);
-  else Launch<BN, false, false, OutT>(ta, tb, p, s);
+                     const GemmParams& p, int sms, cudaStream_t s) {
+  if (ak && bk) Launch<BN, true, true, OutT>(ta, tb, p, sms, s);
+  else if (ak && !bk) Launch<BN, true, false, OutT>(ta, tb, p, sms, s);
+  else if (!ak && bk) Launch<BN, false, true, OutT>(ta, tb, p, sms, s);
+  else Launch<BN, false, false, OutT>(ta, tb, p, sms, s);
 }
 
-// Wave-quantisation heuristic switch, off by default: the 128-wide tile moves 1.33x more
-// operand bytes per FLOP than the 256-wide one. LINGVO_B200_GEMM_AUTO_BN=1 turns it on.
-static bool GemmAutoBn128() {
-  static const bool on = [] {
-    const char* e = getenv("LINGVO_B200_GEMM_AUTO_BN");
-    return e != nullptr && atoi(e) != 0;
-  }();
-  return on;
+// Tile width from the shape: 256 unless N is small, or unless 128-wide tiles finish at
+// least 10 % sooner under the persistent schedule (the busiest CTA runs ceil(tiles / SMs)
+// tiles; a 256-wide tile costs two 128-wide ones). 128-wide tiles move 1.33x more operand
+// bytes per FLOP, hence the margin.
+static bool UseBn256(int64_t G, int64_t M, int64_t N, int sms) {
+  if (N <= 128) return false;
+  const int64_t mt = G * ((M + kBlockM - 1) / kBlockM);
+  const int64_t t256 = mt * ((N + 255) / 256), t128 = mt * ((N + 127) / 128);
+  const int64_t w256 = 2 * ((t256 + sms - 1) / sms), w128 = (t128 + sms - 1) / sms;
+  return w128 * 10 > w256 * 9;
 }
 
 // a: [G, M, K] if a_kmajor else [G, K, M];  b: [G, N, K] if b_kmajor else [G, K, N]
@@ -411,6 +525,14 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
   torch::Tensor out3 = out.dim() == 2 ? out.unsqueeze(0) : out;
   TORCH_CHECK(out3.size(0) == G && out3.size(1) == M && out3.size(2) == N, "gemm_bf16: out shape");
 
+  // The epilogue moves 8 columns per 16-byte access (row_ptrs rows must be 16-byte aligned
+  // as well).
+  auto aligned16 = [](const void* ptr) { return reinterpret_cast<uintptr_t>(ptr) % 16 == 0; };
+  const int64_t vec = fp32 ? 4 : 8;
+  TORCH_CHECK(aligned16(out3.data_ptr()) && out3.stride(1) % vec == 0 &&
+                  (G == 1 || out3.stride(0) % vec == 0),
+              "gemm_bf16: out rows must be 16-byte aligned");
+
   GemmParams p;
   p.G = static_cast<int>(G); p.M = static_cast<int>(M); p.N = static_cast<int>(N);
   p.K = static_cast<int>(K);
@@ -424,6 +546,7 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
   torch::Tensor bias_f;
   if (bias.has_value() && bias->defined()) {
     bias_f = bias->to(torch::kFloat32).contiguous();
+    if (!aligned16(bias_f.data_ptr())) bias_f = bias_f.clone();
     TORCH_CHECK(bias_f.numel() == G * N, "gemm_bf16: bias must be [G, N]");
     p.bias = bias_f.data_ptr<float>();
   }
@@ -433,13 +556,15 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
     TORCH_CHECK(ax.scalar_type() == torch::kBFloat16 && ax.stride(1) == p.ldc &&
                     (G == 1 || ax.stride(0) == p.c_batch) && ax.stride(2) == 1,
                 "gemm_bf16: aux must be bf16 with the same strides as out");
+    TORCH_CHECK(aligned16(ax.data_ptr()), "gemm_bf16: aux must be 16-byte aligned");
     p.aux = reinterpret_cast<const __nv_bfloat16*>(ax.data_ptr());
   }
   if (pre_act.has_value() && pre_act->defined()) {
     torch::Tensor pa = pre_act.value();
     pa = pa.dim() == 2 ? pa.unsqueeze(0) : pa;
     TORCH_CHECK(pa.scalar_type() == torch::kBFloat16 && pa.stride(1) == p.ldc &&
-                    (G == 1 || pa.stride(0) == p.c_batch), "gemm_bf16: pre_act strides");
+                    (G == 1 || pa.stride(0) == p.c_batch) && aligned16(pa.data_ptr()),
+                "gemm_bf16: pre_act strides");
     p.pre_act = pa.data_ptr();
   }
   torch::Tensor rs_f;
@@ -471,22 +596,8 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
 
   if (M == 0 || N == 0 || G == 0) return out;
 
-  // Tile-N: 256 unless N is small — or unless 128-wide tiles quantise better onto the SMs:
-  // an [8192, 2048] output is 512 tiles of 128×256 = 3.88 waves on 132 SMs (4 are paid for),
-  // but 1024 tiles of 128×128 = 7.76 half-cost waves. LINGVO_B200_GEMM_BN=128|256 forces one.
-  bool bn256 = N > 128;
-  if (bn256) {
-    static const int forced = [] {
-      const char* e = getenv("LINGVO_B200_GEMM_BN");
-      return e ? atoi(e) : 0;
-    }();
-    const int sms_q = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
-    const int64_t mt = (M + kBlockM - 1) / kBlockM;
-    const int64_t t256 = G * mt * ((N + 255) / 256), t128 = G * mt * ((N + 127) / 128);
-    const int64_t w256 = 2 * ((t256 + sms_q - 1) / sms_q), w128 = (t128 + sms_q - 1) / sms_q;
-    if (forced == 128) bn256 = false;
-    else if (forced == 0 && GemmAutoBn128() && w128 * 100 <= w256 * 90) bn256 = false;
-  }
+  const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+  const bool bn256 = UseBn256(G, M, N, sms);
   const int bn = bn256 ? 256 : 128;
   TmapArray ta;
   if (a_peer_ptrs.has_value() && a_peer_ptrs->defined()) {
@@ -515,11 +626,11 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
 
   cudaStream_t stream = at::cuda::getCurrentCUDAStream();
   if (bn256) {
-    if (fp32) Dispatch<256, float>(a_kmajor, b_kmajor, ta, tb, p, stream);
-    else Dispatch<256, __nv_bfloat16>(a_kmajor, b_kmajor, ta, tb, p, stream);
+    if (fp32) Dispatch<256, float>(a_kmajor, b_kmajor, ta, tb, p, sms, stream);
+    else Dispatch<256, __nv_bfloat16>(a_kmajor, b_kmajor, ta, tb, p, sms, stream);
   } else {
-    if (fp32) Dispatch<128, float>(a_kmajor, b_kmajor, ta, tb, p, stream);
-    else Dispatch<128, __nv_bfloat16>(a_kmajor, b_kmajor, ta, tb, p, stream);
+    if (fp32) Dispatch<128, float>(a_kmajor, b_kmajor, ta, tb, p, sms, stream);
+    else Dispatch<128, __nv_bfloat16>(a_kmajor, b_kmajor, ta, tb, p, sms, stream);
   }
   return out;
 }
