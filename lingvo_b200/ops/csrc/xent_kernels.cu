@@ -132,15 +132,25 @@ xent_bwd_kernel(__nv_bfloat16* __restrict__ logits, const long long* __restrict_
   }
 }
 
+// Both kernels read (and xent_bwd writes) each row as 16-byte vectors of 8 columns.
+void CheckLogitsAndLabels(const char* op, const torch::Tensor& logits,
+                          const torch::Tensor& labels) {
+  TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == torch::kBFloat16 && logits.dim() == 2 &&
+                  logits.stride(1) == 1,
+              op, ": logits must be a CUDA bf16 [T, V] tensor with unit column stride");
+  TORCH_CHECK(logits.size(1) % 8 == 0 && logits.stride(0) % 8 == 0, op,
+              ": V and the row stride of logits must be multiples of 8");
+  TORCH_CHECK(labels.device() == logits.device() && labels.scalar_type() == torch::kInt64 &&
+                  labels.is_contiguous() && labels.numel() == logits.size(0),
+              op, ": labels must be contiguous int64 [T] on the logits' device");
+}
+
 }  // namespace
 
 std::vector<torch::Tensor> xent_stats(const torch::Tensor& logits, const torch::Tensor& labels) {
-  TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == torch::kBFloat16 && logits.dim() == 2 &&
-              logits.stride(1) == 1);
-  TORCH_CHECK(labels.scalar_type() == torch::kInt64 && labels.is_contiguous());
+  CheckLogitsAndLabels("xent_stats", logits, labels);
   const c10::cuda::CUDAGuard guard(logits.device());
   const int T = static_cast<int>(logits.size(0)), V = static_cast<int>(logits.size(1));
-  TORCH_CHECK(V % 8 == 0 && logits.stride(0) % 8 == 0);
   auto f32 = logits.options().dtype(torch::kFloat32);
   auto lse = torch::empty({T}, f32), tl = torch::empty({T}, f32), sl = torch::empty({T}, f32);
   auto am = torch::empty({T}, logits.options().dtype(torch::kInt64));
@@ -158,7 +168,11 @@ std::vector<torch::Tensor> xent_stats(const torch::Tensor& logits, const torch::
 // In place: logits <- dlogits.
 void xent_bwd(torch::Tensor logits, const torch::Tensor& labels, const torch::Tensor& lse,
               const torch::Tensor& a, const torch::Tensor& b, const torch::Tensor& c) {
-  TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == torch::kBFloat16 && logits.dim() == 2);
+  CheckLogitsAndLabels("xent_bwd", logits, labels);
+  for (const torch::Tensor* t : {&lse, &a, &b, &c})
+    TORCH_CHECK(t->device() == logits.device() && t->scalar_type() == torch::kFloat32 &&
+                    t->is_contiguous() && t->numel() == logits.size(0),
+                "xent_bwd: lse, a, b and c must be contiguous fp32 [T] on the logits' device");
   const c10::cuda::CUDAGuard guard(logits.device());
   const int T = static_cast<int>(logits.size(0)), V = static_cast<int>(logits.size(1));
   if (T == 0) return;

@@ -13,9 +13,10 @@ expert e.
 
 `gate_dispatch` (gate + capacity assignment + peer-store dispatch in one kernel) and
 `scatter_rows` write into *peer* memory through pointer tables and are driven by the exchange
-engine; their math oracle is `core/gshard_layers.Top2GatingIndices` (tested in
-`tests/test_kernels_gpu.py`). The row movers below are plain tensor → tensor and are exposed
-here with `*_ref` oracles like every other op module.
+engine; their math oracle is `top2_gate_ref` below (`core/gshard_layers.Top2GatingIndices`),
+and `tests/test_moe_routing_gpu.py` checks both kernels against it: index, pos, gate and slot
+table exactly, and every expert-buffer row bitwise. The row movers below are plain tensor →
+tensor and are exposed here with `*_ref` oracles like every other op module.
 """
 
 import torch
@@ -93,10 +94,11 @@ def combine_bwd_gate_ref(yc, dy, index, pos, gate, s, g_l, c):
 def top2_gate_ref(logits, paddings, capacity, legacy_mtf_behavior=False):
   """fp32 oracle of the gate half of `moe_gate_dispatch`: → NestedMap(index `[2, G, S]`,
   pos `[2, G, S]`, gate `[2, G, S]`, aux_loss). Thin adapter over
-  `gshard_layers.Top2GatingIndices` (the reference formulation, ref gshard_layers.py:1970)."""
+  `gshard_layers.Top2GatingIndices` (the reference formulation, ref gshard_layers.py:1970).
+  `capacity` is used as given, like the kernel's: no capacity factor enlarges it."""
   from lingvo_b200.core import gshard_layers   # pylint: disable=g-import-not-at-top
   e = logits.shape[-1]
   g = gshard_layers.Top2GatingIndices(
       logits.float(), paddings, e, capacity, torch.float32, 'all', 0.0,
-      legacy_mtf_behavior, 2.0, None)
+      legacy_mtf_behavior, None, None)
   return g

@@ -85,9 +85,25 @@ def test_adafactor_matches_reference(shape, gdtype):
     assert torch.equal(a.compute.data, a.data.bfloat16())
 
 
-def test_lm_head_xent():
+def _ordered_bf16(b):
+  """bf16 bit patterns mapped to integers that are consecutive for adjacent bf16 values."""
+  i = b.contiguous().view(torch.int16).int()
+  return torch.where(i < 0, -(i & 0x7fff), i)
+
+
+def _assert_within_bf16_ulp(got, want, slack):
+  """bf16 `got` is fp32 `want` rounded to bf16 up to one ulp. Where the fp32 terms of an
+  element nearly cancel, `got` may instead be within `slack` of `want`."""
+  ulps = (_ordered_bf16(got) - _ordered_bf16(want.bfloat16())).abs()
+  bad = (ulps > 1) & ~((got.float() - want).abs() <= slack)
+  assert not bool(bad.any()), '%d elements off by more than 1 bf16 ulp' % int(bad.sum())
+
+
+def _check_lm_head_xent(t, m, v):
+  """Fused LM-head xent (GEMM + xent_stats + xent_bwd) vs the fp32 oracle; returns the
+  kernel's and the oracle's stats."""
   from lingvo_b200.ops import xent
-  t, m, v = 512, 256, 2048
+  torch.manual_seed(v)
   x = (torch.randn(t, m, device='cuda') * 0.5).bfloat16().requires_grad_()
   w = (torch.randn(v, m, device='cuda') * 0.1).bfloat16().requires_grad_()
   labels = torch.randint(0, v, (t,), device='cuda')
@@ -100,9 +116,26 @@ def test_lm_head_xent():
   ((ref.soft_xent + ref.z_inc) * wt).sum().backward()
   assert _rel(st.entropy, ref.entropy) < 2e-2
   assert _rel(st.soft_xent, ref.soft_xent) < 2e-2
-  assert (st.argmax == ref.argmax).float().mean() > 0.97
+  # The kernel takes the argmax of bf16 logits: it must be exact wherever the fp32 top two
+  # logits are more than one bf16 ulp apart.
+  top2 = (xr.detach() @ wr.detach().t()).topk(2, dim=-1).values
+  ulp = torch.exp2(torch.floor(torch.log2(top2.abs().max(-1).values)) - 7)
+  clear = (top2[:, 0] - top2[:, 1]) > ulp
+  assert clear.float().mean() > 0.8
+  assert torch.equal(st.argmax[clear], ref.argmax[clear])
   assert _rel(x.grad, xr.grad) < 5e-2
   assert _rel(w.grad, wr.grad) < 5e-2
+  return st, ref
+
+
+def test_lm_head_xent():
+  st, ref = _check_lm_head_xent(512, 256, 2048)
+  assert (st.argmax == ref.argmax).float().mean() > 0.97
+
+
+def test_lm_head_xent_benchmark_vocab():
+  """V = 32000 as in the benchmark: the stats kernel makes 15.6 passes over each row."""
+  _check_lm_head_xent(512, 1024, 32000)
 
 
 def test_ffn_relu():
@@ -120,13 +153,19 @@ def test_ffn_relu():
     assert _rel(a, b) < 3e-2
 
 
-@pytest.mark.parametrize('legacy', [True, False])
-def test_moe_exchange_matches_dense_oracle(legacy):
+@pytest.mark.parametrize('legacy,g,s,m,h', [
+    pytest.param(True, 4, 128, 256, 512, id='True'),
+    pytest.param(False, 4, 128, 256, 512, id='False'),
+    # S = 1024: the gate's position scan carries counts across 4 chunks of 256 tokens.
+    pytest.param(True, 2, 1024, 512, 1024, id='s1024-True'),
+    pytest.param(False, 2, 1024, 512, 1024, id='s1024-False'),
+])
+def test_moe_exchange_matches_dense_oracle(legacy, g, s, m, h):
   """Fused gate+dispatch / expert GEMMs / combine == dense GSEC einsums."""
   from lingvo_b200.core import gshard_layers
   from lingvo_b200.parallel import symm
   torch.manual_seed(1)
-  g, s, m, h, e = 4, 128, 256, 512, 8
+  e = 8
   cap = gshard_layers.ExpertCapacity(s, e, 0, 2.0)
   x = torch.randn(g, s, m, device='cuda').bfloat16().requires_grad_()
   gw = (torch.randn(m, e, device='cuda') * 0.2).requires_grad_()
@@ -532,8 +571,8 @@ def test_beam_topk_kernel_matches_torch_oracle(k, v, dtype):
 
 
 def test_moe_row_movers_match_oracles():
-  """ops/moe.py: token-major combine / gather / gate-gradient kernels vs fp32 oracles."""
-  from lingvo_b200.ops import moe
+  """ops/moe.py: token-major combine / gather / gate-gradient kernels vs fp32 oracles, on
+  random slots (which may collide)."""
   torch.manual_seed(0)
   e, g, c, m, s = 8, 4, 64, 512, 96
   t = g * s
@@ -543,11 +582,47 @@ def test_moe_row_movers_match_oracles():
   pos = torch.randint(0, c, (2, t), device=dev, dtype=torch.int32)
   gate = torch.rand(2, t, device=dev)
   gate[torch.rand(2, t, device=dev) < 0.2] = 0.0                 # dropped choices
+  _check_row_movers(yc, index, pos, gate, s, g, c)
+
+
+@pytest.mark.parametrize('m', [2048, 328])    # 328: not a multiple of the 256-column lane stride
+def test_moe_row_movers_on_gate_kernel_routing(m):
+  """The row movers on the (index, pos, gate) `moe_gate_dispatch` itself produces, at the
+  benchmark's MoE geometry (E = 8, G = 8 groups of S = 1024 tokens, C = 256)."""
+  from lingvo_b200 import ops
+  torch.manual_seed(0)
+  e, g, c, s = 8, 8, 256, 1024
+  t = g * s
+  dev = 'cuda'
+  yc = torch.randn(e, g, c, m, device=dev).bfloat16()
+  logits = torch.randint(-256, 257, (g, s, e), device=dev).float() / 64
+  logits[..., 1] += 2.0                                           # overflows capacity
+  no_peers = torch.zeros(1, dtype=torch.int64, device=dev)
+  index, pos, gate, _ = ops.native().moe_gate_dispatch(logits, None, None, no_peers, c, e, 0, 1,
+                                                        False)
+  index, pos, gate = index.view(2, t), pos.view(2, t), gate.view(2, t)
+  assert bool((gate == 0).any()) and bool((gate != 0).any())
+  _check_row_movers(yc, index, pos, gate, s, g, c)
+
+
+def _check_row_movers(yc, index, pos, gate, s, g, c):
+  """combine / gather_rows to one bf16 ulp of the fp32 oracles, combine_bwd_gate to 1e-5 of
+  the sum of |products|; dropped choices give exactly 0."""
+  from lingvo_b200.ops import moe
+  t, m = index.shape[-1], yc.shape[-1]
+  slack = 2.0**-22 * moe.combine_ref(yc.abs(), index, pos, gate.abs(), s, g, c)
   y = moe.combine(yc, index, pos, gate, s, g, c)
-  assert _rel(y, moe.combine_ref(yc, index, pos, gate, s, g, c)) < 1e-2
+  want = moe.combine_ref(yc, index, pos, gate, s, g, c)
+  assert _rel(y, want) < 1e-2
+  _assert_within_bf16_ulp(y, want, slack)
   ga = moe.gather_rows(yc, index, pos, gate, s, g, c)
-  assert _rel(ga, moe.gather_rows_ref(yc, index, pos, gate, s, g, c)) < 1e-2
-  dy = torch.randn(t, m, device=dev).bfloat16()
+  want = moe.gather_rows_ref(yc, index, pos, gate, s, g, c)
+  assert _rel(ga, want) < 1e-2
+  _assert_within_bf16_ulp(ga, want, 2.0**-22 * moe.gather_rows_ref(yc.abs(), index, pos, gate,
+                                                                   s, g, c))
+  dy = torch.randn(t, m, device=yc.device).bfloat16()
   dg = moe.combine_bwd_gate(yc, dy, index, pos, gate, s, g, c)
   ref = moe.combine_bwd_gate_ref(yc, dy, index, pos, gate, s, g, c)
   assert _rel(dg, ref) < 1e-2 and bool((dg[gate == 0] == 0).all())
+  bound = 1e-5 * moe.combine_bwd_gate_ref(yc.abs(), dy.abs(), index, pos, gate, s, g, c)
+  assert bool(((dg - ref).abs() <= bound).all())
