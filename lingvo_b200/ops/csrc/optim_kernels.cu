@@ -639,7 +639,7 @@ float* ColPartials(const c10::Device& dev, cudaStream_t stream, int64_t slot, in
 // g^2 into `scratch`, optionally sum(w^2) (first step only) and the global sum(g^2).
 // scratch: fp32 [4 + B*R*2 + B*C*2] = acc | rowsum | colsum | fr | fc.
 //   acc[0] = sum(w^2) used now, acc[1] = clipping RMS, acc[2] = sum(w^2) carried to the
-//   next step (persistent), acc[3] unused.
+//   next step (persistent; on a fresh scratch this pass fills it), acc[3] unused.
 void adafactor_stats(const torch::Tensor& w, const torch::Tensor& g, torch::Tensor scratch,
                      int64_t B, int64_t R, int64_t C, bool mult_by_param_scale,
                      bool recompute_wsq, const c10::optional<torch::Tensor>& total_sumsq,
@@ -650,7 +650,10 @@ void adafactor_stats(const torch::Tensor& w, const torch::Tensor& g, torch::Tens
   AfLayout l = Layout(w, scratch, B, R, C);
   if (recompute_wsq) C10_CUDA_CHECK(cudaMemsetAsync(l.acc, 0, sizeof(float) * 4, stream));
   else C10_CUDA_CHECK(cudaMemsetAsync(l.acc + 1, 0, sizeof(float), stream));
-  const int with_w = (recompute_wsq && mult_by_param_scale) ? 1 : 0;
+  // A fresh scratch has no carried Σw² yet: compute it here (also without the parameter
+  // scale, which does not need it) so that acc[2] holds Σw² of the current weights between
+  // this pass and the update, as it does on every later step (the learner's var_norm reads it).
+  const int with_w = recompute_wsq ? 1 : 0;
   float* tot = (total_sumsq.has_value() && total_sumsq->defined())
                    ? total_sumsq->data_ptr<float>() : nullptr;
   const int nblk = static_cast<int>((R + kStatRows - 1) / kStatRows);
@@ -678,7 +681,11 @@ void adafactor_stats(const torch::Tensor& w, const torch::Tensor& g, torch::Tens
     CountLaunch();
   }
   if (tot != nullptr) OrderedSum(bpart.data_ptr<float>(), grid, 2, tot, stream);
-  if (with_w) OrderedSum(bpart.data_ptr<float>() + 1, grid, 2, l.acc, stream);
+  if (with_w) {
+    OrderedSum(bpart.data_ptr<float>() + 1, grid, 2, l.acc, stream);
+    C10_CUDA_CHECK(cudaMemcpyAsync(l.acc + 2, l.acc, sizeof(float), cudaMemcpyDeviceToDevice,
+                                   stream));
+  }
   adafactor_colreduce_kernel<<<dim3(static_cast<unsigned>((C + 255) / 256),
                                     static_cast<unsigned>(B)), 256, 0, stream>>>(
       colpart, l.colsum, (int)C, nblk);
