@@ -15,13 +15,20 @@
 //   groups in a fixed order (bands of kGroupM M-tiles, for L2 reuse), and the
 //   producer runs ahead across tile boundaries, so the ring refills for the next
 //   tile while the consumers run this tile's epilogue;
-// * the fused epilogue (bias, activation, relu-gradient mask / residual add,
-//   per-row scale, accumulate) stages the accumulators through shared memory,
-//   64 columns at a time, and then works on 8 adjacent columns of a row per
-//   thread, so every global load and store is a 16-byte row-contiguous vector.
-//   The store target of every output row can be redirected through a
-//   row-pointer table, which is how the MoE combine (expert GEMM -> NVLink peer
-//   store) is fused.
+// * plain bf16 outputs leave by TMA: each consumer warpgroup applies the fused
+//   epilogue (bias, activation, ReLU-gradient mask / residual add, per-row scale)
+//   in its accumulator layout, writes bf16 into a 64 x 64 swizzled staging slice
+//   and one thread issues a bulk tensor store, so the next tile's MMAs start
+//   without waiting for global memory. The residual / ReLU-mask operand arrives
+//   the same way: TMA loads it into the staging slice ahead of use and the
+//   epilogue overwrites it in place. The epilogue kinds the models use are
+//   compiled as separate specialisations, picked once per tile;
+// * the general epilogue (also accumulate into fp32, pre-activation tap, and
+//   redirected rows) stages fp32 accumulators through shared memory, 64 columns at
+//   a time, and then works on 8 adjacent columns of a row per thread, so every
+//   global load and store is a 16-byte row-contiguous vector. The store target of
+//   every output row can be redirected through a row-pointer table, which is how
+//   the MoE combine (expert GEMM -> NVLink peer store) is fused.
 //
 // Every output tile is computed by one CTA with the same k-block order and wgmma
 // shape as a one-tile-per-CTA launch, so results do not depend on the grid size.
@@ -54,6 +61,9 @@ constexpr int kGroupM = 8;    // M-tiles per rasterisation band
 enum Act : int { kActNone = 0, kActRelu = 1, kActGelu = 2, kActSilu = 3, kActGeluTanh = 4,
                  kActSquaredRelu = 5 };
 enum AuxMode : int { kAuxNone = 0, kAuxReluMask = 1, kAuxAdd = 2 };
+// Epilogue specialisations of the TMA-store path (bias and row scale are uniform branches
+// inside each); kEpiGeneric reads the activation and aux mode from GemmParams.
+enum EpiKind : int { kEpiPlain = 0, kEpiRelu = 1, kEpiAdd = 2, kEpiMask = 3, kEpiGeneric = 4 };
 
 // A operand may be split along K over several tensor maps (one per NVLink peer):
 // the TMA producer then *is* the all-gather (tiles are pulled straight from the
@@ -79,6 +89,7 @@ struct GemmParams {
   int act;
   int aux_mode;
   int accumulate;          // C += result (fp32 out only)
+  int epi;                 // EpiKind (TMA-store path only)
 };
 
 __device__ __forceinline__ float apply_act(float x, int act) {
@@ -163,10 +174,13 @@ struct TileShape {
   static constexpr uint32_t kBBytes = BN * kBlockK * 2;        // 32 KiB (BN=256)
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
   static constexpr uint32_t kRingBytes = kStages * kStageBytes;
-  // fp32 epilogue staging: 64 rows x 64 columns per consumer warpgroup.
+  // Epilogue staging per consumer warpgroup: 64 rows x 64 columns of fp32 (general path),
+  // or two 64 x 64 bf16 slices (TMA-store path, double-buffered).
   static constexpr uint32_t kStagingBytes = 2 * 64 * kEpiCols * 4;
-  static constexpr size_t kSmemBytes = kRingBytes + kStagingBytes + 2 * kStages * 8 + 1024;
+  // full + empty ring barriers, then two aux-load barriers per consumer warpgroup
+  static constexpr size_t kSmemBytes = kRingBytes + kStagingBytes + (2 * kStages + 4) * 8 + 1024;
 };
+constexpr uint32_t kSliceBytes = 64 * kEpiCols * 2;  // one bf16 staging slice (TMA box)
 
 // Tiles are numbered group by group. Inside a group they go in bands of kGroupM M-tiles,
 // M-fastest inside a band: the CTAs of one wave then share a few A panels and B panels in L2.
@@ -194,12 +208,99 @@ __device__ __forceinline__ uint32_t staging_off(int r, int u) {
   return static_cast<uint32_t>(r * (kEpiCols / 4) + (u ^ ((r & 7) << 1))) * 16;
 }
 
-template <int BN, bool kAK, bool kBK, typename OutT>
+// TMA-store epilogue of one warpgroup's 64 x BN block (rows row0.., columns n0..). Slices of
+// 64 columns alternate between the warpgroup's two bf16 staging buffers (`stg`, 128-byte
+// swizzled rows, the layout of the output / aux tensor maps). The first aux slice was loaded
+// during the MMA loop; the next one is loaded as soon as its buffer's store has read it.
+// Per element the arithmetic is that of epilogue_vec8. kAct / kAux < 0: read from p.
+template <int BN, int kAct, int kAux>
+__device__ __forceinline__ void epilogue_tma(const GemmParams& p, float (&acc)[BN / 2],
+                                             const CUtensorMap* tmap_c,
+                                             const CUtensorMap* tmap_aux, uint32_t stg,
+                                             uint32_t aux_bar, uint32_t& aux_par, int row0,
+                                             int n0, int g, int wg) {
+  const int act = kAct >= 0 ? kAct : p.act;
+  const int aux_mode = kAux >= 0 ? kAux : p.aux_mode;
+  const int t = threadIdx.x & 127;
+  const bool leader = t == 0;
+  const int r = (t >> 5) * 16 + ((t & 31) >> 2);   // fragment rows r and r + 8
+  const int q = t & 3;                              // column pair inside an 8-column chunk
+  const float* bias = p.bias ? p.bias + static_cast<long long>(g) * p.N : nullptr;
+  float rs[2] = {1.f, 1.f};
+  if (p.row_scale != nullptr) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+      if (row0 + r + 8 * i < p.M)
+        rs[i] = p.row_scale[static_cast<long long>(g) * p.M + row0 + r + 8 * i];
+  }
+#pragma unroll
+  for (int s = 0; s < BN / kEpiCols; ++s) {
+    const int c0 = n0 + s * kEpiCols;
+    if (c0 >= p.N) break;
+    const uint32_t buf = stg + (s & 1) * kSliceBytes;
+    if (aux_mode != kAuxNone) {
+      mbar_wait(aux_bar + (s & 1) * 8, (aux_par >> (s & 1)) & 1);
+      aux_par ^= 1u << (s & 1);
+    } else {
+      if (leader) tma_store_wait_read<1>();   // the store that last read this buffer
+      named_bar_sync(1 + wg, 128);
+    }
+#pragma unroll
+    for (int n = 0; n < kEpiCols / 8; ++n) {
+      const int col = c0 + 8 * n + 2 * q;
+      float2 b = make_float2(0.f, 0.f);
+      if (bias != nullptr && col < p.N) b = __ldg(reinterpret_cast<const float2*>(bias + col));
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const uint32_t addr = buf + (r + 8 * i) * 128 + ((n ^ (r & 7)) << 4) + q * 4;
+        const int a = 4 * (s * (kEpiCols / 8) + n) + 2 * i;
+        float v0 = acc[a], v1 = acc[a + 1];
+        if (bias != nullptr) { v0 += b.x; v1 += b.y; }
+        v0 = apply_act(v0, act);
+        v1 = apply_act(v1, act);
+        if (aux_mode != kAuxNone) {
+          uint32_t w;
+          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(addr) : "memory");
+          const float2 x = unpack_bf16x2(w);
+          if (aux_mode == kAuxReluMask) {
+            v0 = x.x > 0.f ? v0 : 0.f;
+            v1 = x.y > 0.f ? v1 : 0.f;
+          } else {
+            v0 += x.x;
+            v1 += x.y;
+          }
+        }
+        if (p.row_scale != nullptr) { v0 *= rs[i]; v1 *= rs[i]; }
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_bf16x2(v0, v1)) : "memory");
+      }
+    }
+    fence_proxy_async();
+    named_bar_sync(1 + wg, 128);
+    if (leader) {
+      tma_store_3d(tmap_c, buf, c0, row0, g);
+      tma_store_commit();
+      if (aux_mode != kAuxNone && s + 1 < BN / kEpiCols && c0 + kEpiCols < p.N) {
+        tma_store_wait_read<1>();   // slice s - 1 has left the other buffer
+        const uint32_t nb = aux_bar + ((s + 1) & 1) * 8;
+        mbar_arrive_expect_tx(nb, kSliceBytes);
+        tma_load_3d(stg + ((s + 1) & 1) * kSliceBytes, tmap_aux, nb, c0 + kEpiCols, row0, g);
+      }
+    }
+  }
+}
+
+// kTmaStore: bf16 out through tmap_c (and aux through tmap_aux); otherwise the general
+// epilogue, which ignores both maps.
+template <int BN, bool kAK, bool kBK, typename OutT, bool kTmaStore>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
-                  const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
+                  const __grid_constant__ CUtensorMap tmap_b,
+                  const __grid_constant__ CUtensorMap tmap_c,
+                  const __grid_constant__ CUtensorMap tmap_aux, const GemmParams p) {
   using TS = TileShape<BN>;
   constexpr int kStages = TS::kStages;
+  static_assert(!kTmaStore || sizeof(OutT) == 2, "TMA-store epilogue writes bf16");
+  static_assert(2 * kSliceBytes <= TS::kStagingBytes / 2, "two bf16 slices per warpgroup");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024B alignment for SWIZZLE_128B atoms.
@@ -209,6 +310,7 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
   uint64_t* bars = reinterpret_cast<uint64_t*>(staging + TS::kStagingBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
+  uint64_t* aux_bars = bars + 2 * kStages;   // [wg][buffer]
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -221,6 +323,11 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
   if (threadIdx.x == kNumConsumers) {
     tma_prefetch_desc(&tmaps_a.m[0]);
     tma_prefetch_desc(&tmap_b);
+    if constexpr (kTmaStore) {
+      tma_prefetch_desc(&tmap_c);
+      if (p.aux_mode != kAuxNone) tma_prefetch_desc(&tmap_aux);
+      for (int i = 0; i < 4; ++i) mbar_init(smem_u32(&aux_bars[i]), 1);
+    }
     for (int i = 0; i < kStages; ++i) {
       mbar_init(smem_u32(&full_bar[i]), 1);
       mbar_init(smem_u32(&empty_bar[i]), kNumConsumers / 32);
@@ -276,11 +383,28 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
   setmaxnreg_inc<232>();
   const int wg = warp_idx >> 2;
   const uint32_t stg = smem_u32(staging + wg * (64 * kEpiCols * 4));
+  const uint32_t aux_bar = smem_u32(&aux_bars[2 * wg]);
+  const bool leader = (threadIdx.x & 127) == 0;
+  uint32_t aux_par = 0;   // parity of each staging buffer's aux barrier
   int stage = 0;
   uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const TileCoord tc = tile_coord(tile, tiles_m, tiles_n);
     const int m0 = tc.m_blk * kBlockM, n0 = tc.n_blk * BN, g = tc.g;
+    const int row0 = m0 + wg * 64;
+    // TMA-store path: once the previous tile's stores have read the staging buffers, load
+    // this tile's first aux slice. Issued behind the first k-block's MMAs.
+    auto stage_aux = [&] {
+      if constexpr (kTmaStore) {
+        if (leader && row0 < p.M) {
+          tma_store_wait_read<0>();
+          if (p.aux_mode != kAuxNone) {
+            mbar_arrive_expect_tx(aux_bar, kSliceBytes);
+            tma_load_3d(stg, &tmap_aux, aux_bar, n0, row0, g);
+          }
+        }
+      }
+    };
 
     float acc[BN / 2];
 #pragma unroll
@@ -305,18 +429,47 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
         wgmma_bn<BN, kAK, kBK>(acc, adesc, bdesc);
       }
       wgmma_commit();
+      if (kb == 0) stage_aux();
       wgmma_wait<1>();                 // the previous k-block's MMAs have retired
       __syncwarp();
       if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_stage]));
       prev_stage = stage;
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
+    if (num_k_blocks == 0) stage_aux();
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
     __syncwarp();
     if (num_k_blocks > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_stage]));
 
-    // ============================ epilogue ============================
+    if constexpr (kTmaStore) {
+      if (row0 < p.M) {
+        switch (p.epi) {
+          case kEpiPlain:
+            epilogue_tma<BN, kActNone, kAuxNone>(p, acc, &tmap_c, &tmap_aux, stg, aux_bar,
+                                                 aux_par, row0, n0, g, wg);
+            break;
+          case kEpiRelu:
+            epilogue_tma<BN, kActRelu, kAuxNone>(p, acc, &tmap_c, &tmap_aux, stg, aux_bar,
+                                                 aux_par, row0, n0, g, wg);
+            break;
+          case kEpiAdd:
+            epilogue_tma<BN, kActNone, kAuxAdd>(p, acc, &tmap_c, &tmap_aux, stg, aux_bar,
+                                                aux_par, row0, n0, g, wg);
+            break;
+          case kEpiMask:
+            epilogue_tma<BN, kActNone, kAuxReluMask>(p, acc, &tmap_c, &tmap_aux, stg, aux_bar,
+                                                     aux_par, row0, n0, g, wg);
+            break;
+          default:
+            epilogue_tma<BN, -1, -1>(p, acc, &tmap_c, &tmap_aux, stg, aux_bar, aux_par, row0,
+                                     n0, g, wg);
+        }
+      }
+      continue;
+    }
+
+    // ======================== general epilogue ========================
     // Per 64-column slice: fragments -> staging (fp32), then each thread takes 8 adjacent
     // columns of a row, so every global access is a 16-byte row-contiguous vector.
     const int frow = (warp_idx & 3) * 16 + (lane >> 2);
@@ -375,6 +528,10 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
       }
     }
   }
+  // Shared memory must outlive the bulk stores that read it.
+  if constexpr (kTmaStore) {
+    if (leader) tma_store_wait<0>();
+  }
 }
 
 // ------------------------------------------------------------------ host ----
@@ -420,12 +577,12 @@ CUtensorMap MakeMap(const void* base, int64_t inner, int64_t rows, int64_t group
   return m;
 }
 
-template <int BN, bool kAK, bool kBK, typename OutT>
-static void Launch(const TmapArray& ta, const CUtensorMap& tb, const GemmParams& p,
-                   int sms, cudaStream_t stream) {
+template <int BN, bool kAK, bool kBK, typename OutT, bool kTmaStore>
+static void Launch(const TmapArray& ta, const CUtensorMap& tb, const CUtensorMap& tc,
+                   const CUtensorMap& tx, const GemmParams& p, int sms, cudaStream_t stream) {
   constexpr size_t smem = TileShape<BN>::kSmemBytes;
   static_assert(smem <= 227 * 1024, "GEMM shared memory exceeds the sm_90 limit");
-  auto kern = gemm_wgmma_kernel<BN, kAK, kBK, OutT>;
+  auto kern = gemm_wgmma_kernel<BN, kAK, kBK, OutT, kTmaStore>;
   static bool configured = false;
   if (!configured) {
     C10_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -436,18 +593,19 @@ static void Launch(const TmapArray& ta, const CUtensorMap& tb, const GemmParams&
                         ((p.N + BN - 1) / BN);
   TORCH_CHECK(tiles < (int64_t{1} << 31), "gemm_bf16: too many output tiles");
   const int grid = static_cast<int>(std::min<int64_t>(tiles, sms));
-  kern<<<grid, kNumThreads, smem, stream>>>(ta, tb, p);
+  kern<<<grid, kNumThreads, smem, stream>>>(ta, tb, tc, tx, p);
   CountLaunch();
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
-template <int BN, typename OutT>
+template <int BN, typename OutT, bool kTmaStore>
 static void Dispatch(bool ak, bool bk, const TmapArray& ta, const CUtensorMap& tb,
-                     const GemmParams& p, int sms, cudaStream_t s) {
-  if (ak && bk) Launch<BN, true, true, OutT>(ta, tb, p, sms, s);
-  else if (ak && !bk) Launch<BN, true, false, OutT>(ta, tb, p, sms, s);
-  else if (!ak && bk) Launch<BN, false, true, OutT>(ta, tb, p, sms, s);
-  else Launch<BN, false, false, OutT>(ta, tb, p, sms, s);
+                     const CUtensorMap& tc, const CUtensorMap& tx, const GemmParams& p, int sms,
+                     cudaStream_t s) {
+  if (ak && bk) Launch<BN, true, true, OutT, kTmaStore>(ta, tb, tc, tx, p, sms, s);
+  else if (ak && !bk) Launch<BN, true, false, OutT, kTmaStore>(ta, tb, tc, tx, p, sms, s);
+  else if (!ak && bk) Launch<BN, false, true, OutT, kTmaStore>(ta, tb, tc, tx, p, sms, s);
+  else Launch<BN, false, false, OutT, kTmaStore>(ta, tb, tc, tx, p, sms, s);
 }
 
 // Tile width from the shape: 256 unless N is small, or unless 128-wide tiles finish at
@@ -542,6 +700,7 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
   p.bias = nullptr; p.aux = nullptr; p.row_scale = nullptr; p.pre_act = nullptr;
   p.row_ptrs = nullptr;
   p.nblk_ptrs = nullptr;
+  p.epi = kEpiGeneric;
   p.a_k_per_map = static_cast<int>(K);
   torch::Tensor bias_f;
   if (bias.has_value() && bias->defined()) {
@@ -624,13 +783,34 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
       ? MakeMap(b.data_ptr(), Kb, N, G, b.stride(1), G > 1 ? b.stride(0) : b.stride(1) * b.size(1), bn)
       : MakeMap(b.data_ptr(), N, Kb, G, b.stride(1), G > 1 ? b.stride(0) : b.stride(1) * b.size(1), kBlockK);
 
+  // Plain bf16 outputs (every site but the redirected-row stores) leave through TMA; the
+  // tensor maps clip ragged M / N edges and follow the row and group strides of C.
+  const bool tma_store = !fp32 && p.row_ptrs == nullptr && p.nblk_ptrs == nullptr &&
+                         p.pre_act == nullptr;
+  CUtensorMap tc{}, tx{};
+  if (tma_store) {
+    const int64_t c_group = G > 1 ? p.c_batch : p.ldc * M;
+    tc = MakeMap(p.c, N, M, G, p.ldc, c_group, 64);
+    tx = p.aux ? MakeMap(p.aux, N, M, G, p.ldc, c_group, 64) : tc;
+    if (p.aux_mode == kAuxNone)
+      p.epi = p.act == kActNone ? kEpiPlain : p.act == kActRelu ? kEpiRelu : kEpiGeneric;
+    else if (p.act == kActNone && p.aux_mode == kAuxAdd)
+      p.epi = kEpiAdd;
+    else if (p.act == kActNone && p.aux_mode == kAuxReluMask)
+      p.epi = kEpiMask;
+    else
+      p.epi = kEpiGeneric;
+  }
+
   cudaStream_t stream = at::cuda::getCurrentCUDAStream();
   if (bn256) {
-    if (fp32) Dispatch<256, float>(a_kmajor, b_kmajor, ta, tb, p, sms, stream);
-    else Dispatch<256, __nv_bfloat16>(a_kmajor, b_kmajor, ta, tb, p, sms, stream);
+    if (fp32) Dispatch<256, float, false>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
+    else if (tma_store) Dispatch<256, __nv_bfloat16, true>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
+    else Dispatch<256, __nv_bfloat16, false>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
   } else {
-    if (fp32) Dispatch<128, float>(a_kmajor, b_kmajor, ta, tb, p, sms, stream);
-    else Dispatch<128, __nv_bfloat16>(a_kmajor, b_kmajor, ta, tb, p, sms, stream);
+    if (fp32) Dispatch<128, float, false>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
+    else if (tma_store) Dispatch<128, __nv_bfloat16, true>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
+    else Dispatch<128, __nv_bfloat16, false>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
   }
   return out;
 }
