@@ -711,11 +711,63 @@ void CheckQkv(const torch::Tensor& t, const torch::Tensor& q, const char* name) 
               "flash_attn: ", name, " must be a bf16 [B,L,H,128] view with strides (*, *, 128, 1)");
 }
 
-const int* IntPtr(const c10::optional<torch::Tensor>& t, int64_t B, int64_t L, const char* name) {
-  if (!t.has_value() || !t->defined()) return nullptr;
-  TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kInt32 && t->is_contiguous() &&
-                  t->numel() == B * L, "flash_attn: ", name, " must be int32 [B, L]");
-  return t->data_ptr<int>();
+bool Given(const c10::optional<torch::Tensor>& t) { return t.has_value() && t->defined(); }
+
+const int* IntPtr(const c10::optional<torch::Tensor>& t) {
+  return Given(t) ? t->data_ptr<int>() : nullptr;
+}
+
+// Argument checks of both entry points, made before anything is allocated or launched: every
+// tensor the kernels read or write is on q's device (a host `rel` would otherwise reach the
+// kernel as a host pointer), and seg / pos / lse have the shapes the kernels index. `out`,
+// `d_out` and `lse` are given by the backward only.
+void CheckArgs(const char* op, const torch::Tensor& q, const torch::Tensor& k,
+               const torch::Tensor& v, const c10::optional<torch::Tensor>& rel,
+               const c10::optional<torch::Tensor>& seg, const c10::optional<torch::Tensor>& pos,
+               const torch::Tensor* out = nullptr, const torch::Tensor* d_out = nullptr,
+               const torch::Tensor* lse = nullptr) {
+  TORCH_CHECK(q.is_cuda() && q.dim() == 4 && q.size(3) == kD && q.size(1) % kT == 0 &&
+                  q.size(1) <= 32768,
+              op, ": q must be a CUDA [B, L, H, 128] tensor with L % 128 == 0 and L <= 32768");
+  const int64_t B = q.size(0), L = q.size(1), H = q.size(2);
+  auto on_q = [&](const torch::Tensor& t, const char* name) {
+    TORCH_CHECK(t.device() == q.device(), op, ": ", name, " is on ", t.device(),
+                " but q is on ", q.device());
+  };
+  CheckQkv(q, q, "q");
+  on_q(k, "k");
+  CheckQkv(k, q, "k");
+  on_q(v, "v");
+  CheckQkv(v, q, "v");
+  if (Given(rel)) {
+    on_q(*rel, "rel");
+    TORCH_CHECK(rel->scalar_type() == torch::kFloat32 && rel->dim() == 2 && rel->size(0) == H &&
+                    rel->size(1) == 2 * L - 1, op, ": rel must be fp32 [H, 2L-1]");
+  }
+  for (const auto* t : {&seg, &pos}) {
+    if (!Given(*t)) continue;
+    const char* name = t == &seg ? "segment_ids" : "segment_pos";
+    on_q(**t, name);
+    TORCH_CHECK((*t)->scalar_type() == torch::kInt32 && (*t)->is_contiguous() &&
+                    (*t)->sizes() == torch::IntArrayRef({B, L}),
+                op, ": ", name, " must be contiguous int32 [B, L]");
+  }
+  if (out != nullptr) {
+    on_q(*out, "out");
+    TORCH_CHECK(out->scalar_type() == torch::kBFloat16 && out->is_contiguous() &&
+                    out->sizes() == q.sizes(), op, ": out must be contiguous bf16 [B, L, H, 128]");
+  }
+  if (d_out != nullptr) {
+    on_q(*d_out, "d_out");
+    TORCH_CHECK(d_out->scalar_type() == torch::kBFloat16 && d_out->sizes() == q.sizes(),
+                op, ": d_out must be bf16 [B, L, H, 128]");
+  }
+  if (lse != nullptr) {
+    on_q(*lse, "lse");
+    TORCH_CHECK(lse->scalar_type() == torch::kFloat32 && lse->is_contiguous() &&
+                    lse->sizes() == torch::IntArrayRef({B, H, L}),
+                op, ": lse must be contiguous fp32 [B, H, L]");
+  }
 }
 
 // [B, L/128, 4] int32 block summaries (empty tensor when neither seg nor pos is given).
@@ -751,24 +803,19 @@ std::vector<torch::Tensor> flash_attn_fwd(const torch::Tensor& q, const torch::T
                                           const c10::optional<torch::Tensor>& seg,
                                           const c10::optional<torch::Tensor>& pos, double scale,
                                           bool causal) {
-  TORCH_CHECK(q.dim() == 4 && q.size(3) == kD && q.size(1) % kT == 0,
-              "flash_attn_fwd: needs D == 128 and L % 128 == 0");
-  CheckQkv(q, q, "q"); CheckQkv(k, q, "k"); CheckQkv(v, q, "v");
+  CheckArgs("flash_attn_fwd", q, k, v, rel, seg, pos);
   const int64_t B = q.size(0), L = q.size(1), H = q.size(2);
-  TORCH_CHECK(L <= 32768, "flash_attn: L <= 32768");
   const c10::cuda::CUDAGuard guard(q.device());
   BindContext();
   FwdParams p;
   p.rel = nullptr;
   torch::Tensor relc;
-  if (rel.has_value() && rel->defined()) {
-    TORCH_CHECK(rel->scalar_type() == torch::kFloat32 && rel->dim() == 2 && rel->size(0) == H &&
-                    rel->size(1) == 2 * L - 1, "flash_attn: rel must be fp32 [H, 2L-1]");
+  if (Given(rel)) {
     relc = rel->contiguous();
     p.rel = relc.data_ptr<float>();
   }
-  p.mask.seg = IntPtr(seg, B, L, "segment_ids");
-  p.mask.pos = IntPtr(pos, B, L, "segment_pos");
+  p.mask.seg = IntPtr(seg);
+  p.mask.pos = IntPtr(pos);
   p.mask.causal = causal ? 1 : 0;
   auto blk = BlockMeta(p.mask.seg, p.mask.pos, B, L, q.options());
   p.mask.blk = blk.numel() ? reinterpret_cast<const int4*>(blk.data_ptr<int>()) : nullptr;
@@ -803,11 +850,8 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
                                           const c10::optional<torch::Tensor>& seg,
                                           const c10::optional<torch::Tensor>& pos, double scale,
                                           bool causal, bool need_drel) {
-  CheckQkv(q, q, "q"); CheckQkv(k, q, "k"); CheckQkv(v, q, "v");
+  CheckArgs("flash_attn_bwd", q, k, v, rel, seg, pos, &out, &d_out, &lse);
   const int64_t B = q.size(0), L = q.size(1), H = q.size(2);
-  TORCH_CHECK(q.size(3) == kD && L % kT == 0 && L <= 32768);
-  TORCH_CHECK(out.is_contiguous() && out.sizes() == q.sizes() && out.scalar_type() == torch::kBFloat16);
-  TORCH_CHECK(lse.scalar_type() == torch::kFloat32 && lse.is_contiguous() && lse.numel() == B * H * L);
   const c10::cuda::CUDAGuard guard(q.device());
   BindContext();
   auto d_o = d_out.contiguous();
@@ -826,9 +870,7 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
   BwdParams p;
   p.rel = nullptr;
   torch::Tensor relc, drel;
-  if (rel.has_value() && rel->defined()) {
-    TORCH_CHECK(rel->scalar_type() == torch::kFloat32 && rel->dim() == 2 && rel->size(0) == H &&
-                rel->size(1) == 2 * L - 1);
+  if (Given(rel)) {
     relc = rel->contiguous();
     p.rel = relc.data_ptr<float>();
   }
@@ -837,8 +879,8 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
   } else {
     drel = torch::empty({0}, lse.options());
   }
-  p.mask.seg = IntPtr(seg, B, L, "segment_ids");
-  p.mask.pos = IntPtr(pos, B, L, "segment_pos");
+  p.mask.seg = IntPtr(seg);
+  p.mask.pos = IntPtr(pos);
   p.mask.causal = causal ? 1 : 0;
   auto blk = BlockMeta(p.mask.seg, p.mask.pos, B, L, q.options());
   p.mask.blk = blk.numel() ? reinterpret_cast<const int4*>(blk.data_ptr<int>()) : nullptr;
