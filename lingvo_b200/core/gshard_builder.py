@@ -497,18 +497,6 @@ class SelfAttentionLayer(_BuilderLayer):
         o = attention_ops.flash_attention(q, k, v, rel, segment_id, segment_pos, 1.0, causal)
         out = gemm.linear(o.reshape(bsz, l, h * d), wo.to(x.dtype), residual=residual)
         return out, torch.zeros((), device=x.device, dtype=torch.float32)
-    if (simple and self.params.relative_bias and
-        b.relative_attention_use_universal_1d_position):
-      from lingvo_b200.ops import attention as attention_ops
-      rel = self._RelTable(theta, l, x.device)
-      if attention_ops.rel_bias_attention_supported(q, k, rel, drop):
-        # cuDNN fused attention + our bias-build / wgmma bias-gradient kernels.
-        mask = self._Mask(segment_id, segment_pos, torch.float32)
-        o = attention_ops.rel_bias_attention(
-            q, k, v, rel, mask, 1.0,
-            causal=self.params.decoder and not b.decoder_skip_causal_mask)
-        out = gemm.linear(o.reshape(bsz, l, h * d), wo.to(x.dtype), residual=residual)
-        return out, torch.zeros((), device=x.device, dtype=torch.float32)
     bias = self._Bias(theta, segment_id, segment_pos,
                       x.dtype if (simple and x.is_cuda) else torch.float32)
     o = _AttentionCore(q, k, v, bias, b.atten_logit_cap,

@@ -14,7 +14,6 @@ Dispatch:
 
 from __future__ import annotations
 
-import os
 from typing import Optional
 
 import torch
@@ -85,103 +84,6 @@ def _RelToeplitz(rel, l):
   return rel.flip(-1).unfold(-1, l, 1).flip(1)
 
 
-def rel_bias_attention_ref(q, k, v, rel, mask=None, scale=1.0):
-  """fp32 oracle: softmax(scale·q·kᵀ + rel[h, i-j+L-1] + mask[b,i,j])·v."""
-  l = q.shape[1]
-  bias = _RelToeplitz(rel.float(), l).unsqueeze(0)
-  if mask is not None:
-    bias = bias + mask.float().reshape(-1, 1, l, l)
-  return attention_ref(q, k, v, bias, scale)
-
-
-# Whether this cuDNN build accepts an additive bias together with its own causal mask
-# (it then skips the fully-masked upper-triangular tiles). Probed on first use.
-_CUDNN_BIAS_PLUS_CAUSAL = {'ok': None}
-
-
-def _CudnnFwd(qt, kt, vt, bias, scale, causal):
-  use = causal and _CUDNN_BIAS_PLUS_CAUSAL['ok'] is not False
-  if use:
-    try:
-      res = torch.ops.aten._scaled_dot_product_cudnn_attention(
-          qt, kt, vt, bias, True, 0.0, True, False, scale=scale)
-      _CUDNN_BIAS_PLUS_CAUSAL['ok'] = True
-      return res, True
-    except RuntimeError:
-      if _CUDNN_BIAS_PLUS_CAUSAL['ok'] is True:
-        raise
-      _CUDNN_BIAS_PLUS_CAUSAL['ok'] = False
-  return torch.ops.aten._scaled_dot_product_cudnn_attention(
-      qt, kt, vt, bias, True, 0.0, False, False, scale=scale), False
-
-
-class _RelBiasAttnFn(torch.autograd.Function):
-  """Flash attention with a learned Toeplitz bias.
-
-  forward : `build_rel_bias` (ours) → cuDNN fused attention (library, like
-            cuBLAS for plain GEMMs) producing O and the log-sum-exp.
-  backward: cuDNN fused backward for dQ/dK/dV + `rel_bias_grad` (our wgmma
-            kernel) for the bias-table gradient, which cuDNN cannot produce.
-  """
-
-  @staticmethod
-  def forward(ctx, q, k, v, rel, mask, scale, causal):
-    from lingvo_b200 import ops
-    nat = ops.native()
-    b, l, h, d = q.shape
-    bias = nat.build_rel_bias(rel.float().contiguous(), mask, b)
-    qt, kt, vt = q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)
-    res, cudnn_causal = _CudnnFwd(qt, kt, vt, bias, scale, causal)
-    out, lse = res[0], res[1]
-    ctx.save_for_backward(q, k, v, out, lse, bias, res[2], res[3], res[6], res[7])
-    ctx.meta = (res[4], res[5], scale, causal, cudnn_causal)
-    return out.transpose(1, 2)
-
-  @staticmethod
-  def backward(ctx, d_o):
-    from lingvo_b200 import ops
-    nat = ops.native()
-    q, k, v, out, lse, bias, cq, ck, seed, off = ctx.saved_tensors
-    max_q, max_k, scale, causal, cudnn_causal = ctx.meta
-    b, l, h, d = q.shape
-    d_o = d_o.contiguous()                                   # [B, L, H, D]
-    dq, dk, dv = torch.ops.aten._scaled_dot_product_cudnn_attention_backward(
-        d_o.transpose(1, 2), q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2),
-        out, lse, seed, off, bias, cq, ck, max_q, max_k, 0.0, cudnn_causal, scale=scale)
-    drel = None
-    if ctx.needs_input_grad[3]:
-      lse3 = lse.reshape(b, h, l).float().contiguous()
-      drel = nat.rel_bias_grad(q, k, v, d_o, out, lse3, bias, scale, causal)
-    return (dq.transpose(1, 2), dk.transpose(1, 2), dv.transpose(1, 2), drel,
-            None, None, None)
-
-
-def rel_bias_attention_supported(q, k, rel, dropout_prob=0.0):
-  from lingvo_b200 import ops
-  return (ops.use_cuda_kernels(q) and q.dtype == torch.bfloat16 and
-          q.shape[-1] == 128 and q.shape[1] % 128 == 0 and
-          q.shape[1] == k.shape[1] and q.shape[2] == k.shape[2] and
-          not dropout_prob and rel.shape[-1] == 2 * q.shape[1] - 1)
-
-
-def rel_bias_attention(q, k, v, rel, mask=None, scale=1.0, causal=False):
-  """`[B,L,H,D]` self-attention with bias `rel[h, i-j+L-1] + mask[b,i,j]`.
-
-  `causal=True` promises that `mask` hides every j > i, which lets the bias
-  gradient kernel skip the upper-triangular tiles.
-  """
-  if not rel_bias_attention_supported(q, k, rel):
-    return rel_bias_attention_ref(q, k, v, rel, mask, scale).to(q.dtype)
-  if mask is not None:
-    mask = mask.reshape(-1, q.shape[1], q.shape[1])
-  def _View(t):   # [B,L,H,D] view with strides (*, *, D, 1), 16-byte aligned rows
-    ok = (t.stride(3) == 1 and t.stride(2) == t.shape[3] and t.stride(1) % 8 == 0 and
-          t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0)
-    return t if ok else t.contiguous()
-  return _RelBiasAttnFn.apply(_View(q), _View(k), _View(v), rel, mask,
-                              float(scale), bool(causal))
-
-
 # ------------------------------------------------------------ wgmma flash attention ----
 def flash_attention_ref(q, k, v, rel=None, seg=None, pos=None, scale=1.0, causal=False):
   """fp32 oracle of `flash_attention`: packed-input mask built from segment ids / positions
@@ -229,7 +131,6 @@ def flash_attention_supported(q, k, dropout_prob=0.0):
   from lingvo_b200 import ops
   mod = ops.native(required=False) if q.is_cuda else None
   return (mod is not None and hasattr(mod, '_has_flash_attn') and
-          os.environ.get('LINGVO_B200_ATTN', 'flash') == 'flash' and
           ops.use_cuda_kernels(q) and q.dtype == torch.bfloat16 and q.dim() == 4 and
           q.shape[-1] == 128 and q.shape[1] % 128 == 0 and q.shape == k.shape and
           not dropout_prob)

@@ -11,7 +11,7 @@
 //       stored straight into every peer's replica of the parameters.
 //   tp_reduce_slabs : owner-side sum of the W partial slabs written by the
 //       row-pointer epilogue of the tensor-parallel GEMM (GEMM -> reduce-scatter).
-// Flags (moe_signal / moe_wait) order the phases across ranks.
+// The device-counter flags of moe_sync order the phases across ranks.
 
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>

@@ -27,13 +27,9 @@
 
 #include "ptx.cuh"
 #include "registry.h"
+#include "tmap.h"
 
 namespace lb {
-
-CUtensorMap MakeMap(const void* base, int64_t inner, int64_t rows, int64_t groups,
-                    int64_t row_stride, int64_t group_stride, int box_rows,
-                    CUtensorMapDataType dt = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, int elem_bytes = 2);
-
 namespace {
 
 constexpr int kT = 128;                      // tile edge (queries / keys)
@@ -783,17 +779,6 @@ torch::Tensor BlockMeta(const int* seg, const int* pos, int64_t B, int64_t L,
   return out;
 }
 
-void BindContext() {
-  static thread_local bool bound = false;
-  if (bound) return;
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(at::cuda::getCurrentCUDAStream(), &cap);
-  if (cap == cudaStreamCaptureStatusNone) {
-    C10_CUDA_CHECK(cudaFree(nullptr));
-    bound = true;
-  }
-}
-
 }  // namespace
 
 // Returns (out [B,L,H,D] bf16, lse [B,H,L] fp32).
@@ -806,7 +791,6 @@ std::vector<torch::Tensor> flash_attn_fwd(const torch::Tensor& q, const torch::T
   CheckArgs("flash_attn_fwd", q, k, v, rel, seg, pos);
   const int64_t B = q.size(0), L = q.size(1), H = q.size(2);
   const c10::cuda::CUDAGuard guard(q.device());
-  BindContext();
   FwdParams p;
   p.rel = nullptr;
   torch::Tensor relc;
@@ -853,7 +837,6 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
   CheckArgs("flash_attn_bwd", q, k, v, rel, seg, pos, &out, &d_out, &lse);
   const int64_t B = q.size(0), L = q.size(1), H = q.size(2);
   const c10::cuda::CUDAGuard guard(q.device());
-  BindContext();
   auto d_o = d_out.contiguous();
   CheckQkv(d_o, q, "dO");
   auto stream = at::cuda::getCurrentCUDAStream();

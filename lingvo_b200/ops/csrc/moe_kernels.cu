@@ -18,8 +18,9 @@
 // moe_scatter_rows: the same slot-major peer store for the backward pass
 // (d_out = gate * dy routed back to the experts).
 // moe_combine / moe_combine_bwd / moe_gather_rows: token-major local gathers.
-// moe_signal / moe_wait: release/acquire flags at system scope replacing the
-// collective's implicit barrier.
+// moe_sync: release/acquire flags at system scope replacing the collective's
+// implicit barrier; the sequence number is a device counter, so it can be
+// replayed from a CUDA graph.
 
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -393,30 +394,10 @@ __global__ void moe_gather_rows_kernel(const __nv_bfloat16* __restrict__ src,
   }
 }
 
-// flags[channel][src_rank] on every peer <- seq  (release at system scope)
-__global__ void moe_signal_kernel(const long long* __restrict__ peer_flags, int world, int rank,
-                                  int channel, int seq) {
-  const int r = threadIdx.x;
-  if (r < world) {
-    __threadfence_system();
-    int* f = reinterpret_cast<int*>(peer_flags[r]) + channel * world + rank;
-    st_release_sys(f, seq);
-  }
-}
-__global__ void moe_wait_kernel(const int* __restrict__ flags, int world, int channel, int seq) {
-  const int r = threadIdx.x;
-  if (r < world) {
-    const int* f = flags + channel * world + r;
-    while (ld_acquire_sys(f) < seq) {
-      __nanosleep(64);
-    }
-  }
-  __syncthreads();
-}
-
-// Device-counter flavour: one kernel = signal every peer, then wait for every peer. The
-// sequence number lives in device memory (`counter[channel]`, bumped by the kernel), so the
-// launch has no step-dependent argument and can be replayed from a CUDA graph.
+// One kernel = signal every peer (flags[channel][src_rank] <- seq, release at system
+// scope), then wait for every peer. The sequence number lives in device memory
+// (`counter[channel]`, bumped by the kernel), so the launch has no step-dependent argument
+// and can be replayed from a CUDA graph.
 __global__ void moe_sync_kernel(const long long* __restrict__ peer_flags,
                                 const int* __restrict__ flags, int* __restrict__ counters,
                                 int world, int rank, int channel) {
@@ -565,29 +546,12 @@ torch::Tensor moe_gather_rows(const torch::Tensor& src, const torch::Tensor& ind
   return out;
 }
 
-void moe_signal(const torch::Tensor& peer_flags, int64_t world, int64_t rank, int64_t channel,
-                int64_t seq) {
-  const c10::cuda::CUDAGuard guard(peer_flags.device());
-  moe_signal_kernel<<<1, 32, 0, at::cuda::getCurrentCUDAStream()>>>(
-      reinterpret_cast<long long*>(peer_flags.data_ptr<int64_t>()), (int)world, (int)rank, (int)channel, (int)seq);
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
-  CountLaunch();
-}
 void moe_sync(const torch::Tensor& peer_flags, const torch::Tensor& flags, torch::Tensor counters,
               int64_t world, int64_t rank, int64_t channel) {
   TORCH_CHECK(counters.is_cuda() && counters.scalar_type() == torch::kInt32);
   const c10::cuda::CUDAGuard guard(flags.device());
   moe_sync_kernel<<<1, 32, 0, at::cuda::getCurrentCUDAStream()>>>(
       reinterpret_cast<const long long*>(peer_flags.data_ptr<int64_t>()), flags.data_ptr<int>(), counters.data_ptr<int>(), (int)world, (int)rank, (int)channel);
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
-  CountLaunch();
-}
-
-void moe_wait(const torch::Tensor& flags, int64_t world, int64_t channel, int64_t seq) {
-  const c10::cuda::CUDAGuard guard(flags.device());
-  moe_wait_kernel<<<1, 32, 0, at::cuda::getCurrentCUDAStream()>>>(flags.data_ptr<int>(),
-                                                                   (int)world, (int)channel,
-                                                                   (int)seq);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
   CountLaunch();
 }
@@ -629,8 +593,6 @@ LB_REGISTER(moe) {
   m.def("moe_combine", &lb::moe_combine);
   m.def("moe_combine_bwd_gate", &lb::moe_combine_bwd_gate);
   m.def("moe_gather_rows", &lb::moe_gather_rows);
-  m.def("moe_signal", &lb::moe_signal);
-  m.def("moe_wait", &lb::moe_wait);
   m.def("moe_sync", &lb::moe_sync);
   m.def("symm_alloc", &lb::symm_alloc);
   m.def("symm_export", &lb::symm_export);

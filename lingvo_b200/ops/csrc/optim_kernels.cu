@@ -779,18 +779,6 @@ void small_sumsq(const torch::Tensor& table, torch::Tensor out) {
   CountLaunch();
 }
 
-// One-call form (stats + update) kept for callers that do not need the global norm.
-void adafactor_factored(torch::Tensor w, const torch::Tensor& g, torch::Tensor vr,
-                        torch::Tensor vc, torch::Tensor scratch,
-                        const c10::optional<torch::Tensor>& w_bf16, int64_t B, int64_t R,
-                        int64_t C, bool vr_is_rows, double lr, double decay, double eps1,
-                        double eps2, double clip, bool mult_by_param_scale,
-                        const c10::optional<torch::Tensor>& grad_scale, bool recompute_wsq) {
-  adafactor_stats(w, g, scratch, B, R, C, mult_by_param_scale, recompute_wsq, c10::nullopt, 0);
-  adafactor_update(w, g, vr, vc, scratch, w_bf16, B, R, C, vr_is_rows, lr, decay, eps1, eps2, clip,
-                   mult_by_param_scale, grad_scale, recompute_wsq, c10::nullopt);
-}
-
 void adam_flat(torch::Tensor w, const torch::Tensor& g, torch::Tensor m, torch::Tensor v,
                const c10::optional<torch::Tensor>& w_bf16,
                const c10::optional<torch::Tensor>& grad_scale_t, double lr_t, double b1, double b2,
@@ -825,7 +813,6 @@ void adam_flat(torch::Tensor w, const torch::Tensor& g, torch::Tensor m, torch::
 
 LB_REGISTER(optim) {
   m.attr("_has_optim") = true;
-  m.def("adafactor_factored", &lb::adafactor_factored);
   m.def("adafactor_stats", &lb::adafactor_stats);
   m.def("adafactor_update", &lb::adafactor_update);
   m.def("adafactor_small", &lb::adafactor_small);

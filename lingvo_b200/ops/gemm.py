@@ -66,7 +66,7 @@ def gemm(a, b, a_kmajor=True, b_kmajor=True, bias=None, act=0, aux=None,
          aux_mode=0, row_scale=None, out=None, out_fp32=False,
          accumulate=False, pre_act=None, row_ptrs=None, nblk_ptrs=None,
          a_peer_ptrs=None, nblk_ld=0):
-  """C[g] = epi(A[g] · B[g]^T); see csrc/gemm_tcgen05.cu for operand layouts."""
+  """C[g] = epi(A[g] · B[g]^T); see csrc/gemm_wgmma.cu for operand layouts."""
   act = ACT_IDS[act] if not isinstance(act, int) else act
   if not ops.use_cuda_kernels(a, b):
     y = gemm_ref(a, b, a_kmajor, b_kmajor, bias, act, aux, aux_mode, row_scale,

@@ -50,26 +50,6 @@ def Invalidate():
       buf[2:3] = var.data.float().square().sum().reshape(1)
 
 
-def adafactor_factored(var, grad, vr, vc, d0, d1, lr, decay, eps1, eps2, clip,
-                       mult_by_param_scale, grad_scale=None):
-  """In-place Adafactor step; factored dims (d0, d1) must be the last two.
-
-  d0 is the reference's `vr_axis` (largest dim): `vr` = mean over d0.
-  """
-  nd = var.dim()
-  assert sorted((d0, d1)) == [nd - 2, nd - 1]
-  r, c = var.shape[-2], var.shape[-1]
-  b = var.numel() // (r * c)
-  vr_is_rows = (d0 == nd - 1)   # vr = mean over C → per-row vector [B, R]
-  scratch, fresh = _Scratch(var, 16 + 2 * (b * r + 4) + 2 * (b * c + 4))
-  g = grad if grad.is_contiguous() else grad.contiguous()
-  compute = getattr(var, 'compute', None)
-  ops.native().adafactor_factored(
-      var.data, g, vr, vc, scratch, compute.data if compute is not None else None,
-      b, r, c, vr_is_rows, float(lr), float(decay), float(eps1), float(eps2),
-      float(clip), bool(mult_by_param_scale), grad_scale, fresh)
-
-
 def _KernelGrad(grad, b):
   """The fused kernels take a contiguous gradient or (for a single matrix) a column slice of
   a wider row-major matrix — e.g. dwq/dwk/dwv as views of the fused qkv weight gradient —

@@ -196,52 +196,6 @@ def test_moe_exchange_matches_dense_oracle(legacy, g, s, m, h):
   assert _rel(wo.grad, wor.grad) < 5e-2
 
 
-@pytest.mark.parametrize('causal', [True, False])
-def test_rel_bias_attention_matches_oracle(causal):
-  """cuDNN fwd/bwd + our build_rel_bias / wgmma rel_bias_grad vs fp32 oracle."""
-  from lingvo_b200.ops import attention as A
-  torch.manual_seed(0)
-  dev = torch.device('cuda')
-  b, l, h, d = 2, 256, 4, 128
-  q = (torch.randn(b, l, h, d, device=dev) * 0.3).bfloat16().requires_grad_()
-  k = (torch.randn(b, l, h, d, device=dev) * 0.3).bfloat16().requires_grad_()
-  v = torch.randn(b, l, h, d, device=dev).bfloat16().requires_grad_()
-  rel = (torch.randn(h, 2 * l - 1, device=dev) * 0.5).requires_grad_()
-  seg = torch.ones(b, l, device=dev, dtype=torch.int32)
-  seg[1, 100:] = 2                                  # packed: two segments in row 1
-  not_vis = seg.unsqueeze(-1) != seg.unsqueeze(-2)
-  if causal:
-    not_vis = not_vis | torch.triu(torch.ones(l, l, dtype=torch.bool, device=dev), 1)
-  mask = not_vis.float() * -1e9
-  do = torch.randn(b, l, h, d, device=dev).bfloat16()
-  assert A.rel_bias_attention_supported(q, k, rel)
-  o = A.rel_bias_attention(q, k, v, rel, mask, 1.0, causal=causal)
-  o.backward(do)
-  got = [o.detach().float(), q.grad.float(), k.grad.float(), v.grad.float(), rel.grad.clone()]
-  for t in (q, k, v, rel):
-    t.grad = None
-  qr, kr, vr = (t.detach().float().requires_grad_() for t in (q, k, v))
-  relr = rel.detach().clone().requires_grad_()
-  o_ref = A.rel_bias_attention_ref(qr, kr, vr, relr, mask, 1.0)
-  o_ref.backward(do.float())
-  want = [o_ref.detach(), qr.grad, kr.grad, vr.grad, relr.grad]
-  for name, g, w in zip(['o', 'dq', 'dk', 'dv', 'drel'], got, want):
-    err = float((g - w).norm() / w.norm().clamp_min(1e-6))
-    assert err < 2e-2, (name, err)
-
-
-def test_build_rel_bias():
-  from lingvo_b200 import ops
-  from lingvo_b200.ops import attention as A
-  dev = torch.device('cuda')
-  h, l, b = 3, 64, 2
-  rel = torch.randn(h, 2 * l - 1, device=dev)
-  mask = torch.randn(b, l, l, device=dev)
-  got = ops.native().build_rel_bias(rel, mask, b).float()
-  want = A._RelToeplitz(rel, l).unsqueeze(0) + mask.unsqueeze(1)
-  torch.testing.assert_close(got, want.bfloat16().float(), atol=2e-2, rtol=2e-2)
-
-
 @pytest.mark.parametrize('causal', [False, True])
 @pytest.mark.parametrize('dtype', [torch.bfloat16, torch.float32])
 def test_glu_dwconv1d_kernel(causal, dtype):
@@ -466,7 +420,7 @@ def test_gate_logits_pass_adds_the_other_branch_gradient():
     (2, 384, 2, True, 3, True),
     (2, 512, 4, False, 4, False),
 ])
-def test_flash_attention_tcgen05_matches_fp32_oracle(b, l, h, use_rel, segs, causal):
+def test_flash_attention_wgmma_matches_fp32_oracle(b, l, h, use_rel, segs, causal):
   """Our flash attention (fwd, dQ/dK/dV, d rel-bias) vs the plain fp32 softmax oracle, with
   packed segments + padding, causal and bidirectional."""
   from lingvo_b200.ops import attention as A

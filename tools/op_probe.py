@@ -53,19 +53,6 @@ def main():
   out['gate_logits_fwd_torch'] = {'us': Time(ref)}
   out['gate_logits_bwd_torch'] = {
       'us': Time(lambda: torch.autograd.grad(yr, [x, gw], dl, retain_graph=True))}
-  # relative-bias attention: cuDNN fwd/bwd + build_rel_bias / attn_delta / rel_bias_grad (ours)
-  from lingvo_b200.ops import attention as A
-  b, l, h, d = 8, 1024, 16, 128
-  q = (torch.randn(b, l, h, d, device='cuda') * 0.3).to(torch.bfloat16).requires_grad_()
-  k = (torch.randn(b, l, h, d, device='cuda') * 0.3).to(torch.bfloat16).requires_grad_()
-  v = torch.randn(b, l, h, d, device='cuda').to(torch.bfloat16).requires_grad_()
-  rel = (torch.randn(h, 2 * l - 1, device='cuda') * 0.5).requires_grad_()
-  mask = (torch.triu(torch.ones(l, l, device='cuda'), 1).unsqueeze(0).expand(b, l, l) * -1e9).contiguous()
-  o = A.rel_bias_attention(q, k, v, rel, mask, 1.0, causal=True)
-  do = torch.randn_like(o)
-  out['rel_bias_attention_fwd'] = {'us': Time(lambda: A.rel_bias_attention(q, k, v, rel, mask, 1.0, causal=True))}
-  out['rel_bias_attention_bwd'] = {
-      'us': Time(lambda: torch.autograd.grad(o, [q, k, v, rel], do, retain_graph=True))}
   print(json.dumps(out, indent=1))
 
 

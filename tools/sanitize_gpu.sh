@@ -8,7 +8,7 @@ set -u
 mkdir -p gpurun_out
 SAN=${COMPUTE_SANITIZER:-/usr/local/cuda/bin/compute-sanitizer}
 TESTS=${SANITIZE_TESTS:-"tests/test_kernels_gpu.py tests/test_gemm_gpu.py"}
-SELECT=${SANITIZE_K:-"rms_norm or layer_norm or gate_logits or adafactor or lm_head or ffn_relu or layouts or build_rel_bias"}
+SELECT=${SANITIZE_K:-"rms_norm or layer_norm or gate_logits or adafactor or lm_head or ffn_relu or layouts"}
 rc=0
 for tool in ${SANITIZE_TOOLS:-memcheck racecheck synccheck initcheck}; do
   log=gpurun_out/sanitizer_${tool}.log
