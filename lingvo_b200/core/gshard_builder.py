@@ -487,11 +487,12 @@ class SelfAttentionLayer(_BuilderLayer):
     simple = (not b.atten_logit_cap) and b.attention_extra_logit is None
     drop = b.attention_dropout_prob if not self.do_eval else 0.0
     toeplitz = (not self.params.relative_bias) or b.relative_attention_use_universal_1d_position
-    if simple and toeplitz and hk == h:
+    if simple and toeplitz:
       from lingvo_b200.ops import attention as attention_ops
       if attention_ops.flash_attention_supported(q, k, drop):
         # Our wgmma flash attention: bias table + packed-input mask applied in registers,
-        # dRel folded into the backward; output already `[B, L, H, D]`.
+        # dRel folded into the backward; grouped / multi-query KV heads are read in place;
+        # output already `[B, L, H, D]`.
         rel = self._RelTable(theta, l, x.device) if self.params.relative_bias else None
         causal = self.params.decoder and not b.decoder_skip_causal_mask
         o = attention_ops.flash_attention(q, k, v, rel, segment_id, segment_pos, 1.0, causal)

@@ -84,6 +84,7 @@ class DenseLmTemplate(base_model_params.SingleTaskModelParams):
   ATTENTION_KEY_VALUE_DIM = 128
   MODEL_DIM = 8192
   NUM_HEADS = 128
+  NUM_KV_HEADS = None        # grouped-query / multi-query attention; None = NUM_HEADS
   NUM_TRANSFORMER_LAYERS = 32
   LABEL_SMOOTHING = 0.0
   VOCAB_SIZE = 32000
@@ -117,6 +118,7 @@ class DenseLmTemplate(base_model_params.SingleTaskModelParams):
         model_dim_reshape_segments=self.MODEL_DIM_RESHAPE_SEGMENTS,
         model_dim=self.MODEL_DIM,
         attention_num_heads=self.NUM_HEADS,
+        attention_num_memory_heads=self.NUM_KV_HEADS,
         ff_dim=self.HIDDEN_DIM,
         attention_combine_dims=True)
 
@@ -452,6 +454,13 @@ class MoELm8E(MoELmTemplate):
   NUM_EXPERTS = 8
   BATCH_SIZE_PER_GPU = 8
   TRAIN_STEPS_PER_LOOP = 20
+
+
+@model_registry.RegisterSingleTaskModel
+class MoELm8EKv4(MoELm8E):
+  """MoELm8E with grouped-query attention: 16 query heads share 4 KV heads (wk, wv
+  [2048, 512]), which makes the decoding KV cache 4x smaller."""
+  NUM_KV_HEADS = 4
 
 
 @model_registry.RegisterSingleTaskModel

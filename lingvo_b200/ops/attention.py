@@ -132,13 +132,18 @@ def flash_attention_supported(q, k, dropout_prob=0.0):
   mod = ops.native(required=False) if q.is_cuda else None
   return (mod is not None and hasattr(mod, '_has_flash_attn') and
           ops.use_cuda_kernels(q) and q.dtype == torch.bfloat16 and q.dim() == 4 and
-          q.shape[-1] == 128 and q.shape[1] % 128 == 0 and q.shape == k.shape and
-          not dropout_prob)
+          q.shape[-1] == 128 and q.shape[1] % 128 == 0 and k.dim() == 4 and
+          k.shape[:2] == q.shape[:2] and k.shape[3] == 128 and k.shape[2] >= 1 and
+          q.shape[2] % k.shape[2] == 0 and not dropout_prob)
 
 
 def flash_attention(q, k, v, rel=None, seg=None, pos=None, scale=1.0, causal=False):
   """`[B,L,H,128]` self-attention, bias `rel[h, i-j+L-1]` (fp32 `[H, 2L-1]`, optional) and
   the packed-input mask from int32 `seg` / `pos` `[B, L]` (optional). Returns `[B,L,H,128]`.
+
+  k and v are `[B,L,Hk,128]` with Hk dividing H: grouped-query (Hk < H) or multi-query
+  (Hk = 1) attention, where query head h reads KV head h // (H/Hk). Their gradients keep Hk
+  heads, each summed over its group.
 
   `causal=True` additionally assumes positions grow with the index inside a segment (packed
   LM inputs), which lets both kernels skip the key blocks above the diagonal.

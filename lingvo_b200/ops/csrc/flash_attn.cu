@@ -15,9 +15,14 @@
 // operand (rows = M/N index) or an MN-major operand (rows = K index) by changing only the
 // descriptor and the wgmma transpose bit, so no transposes are ever materialised.
 //
-// Layouts: q,k,v,dO [B, L, H, D=128] bf16 views (strides (*, *, D, 1));  O, dK, dV
-// [B, L, H, D] contiguous bf16;  dq_part [Jc, B, L, H, D] fp32;  lse, delta [B, H, L] fp32;
-// rel / drel [H, 2L-1] fp32;  segment ids / positions [B, L] int32 (optional).
+// Grouped-query / multi-query attention: k and v may have Hk heads with H % Hk == 0; query
+// head h reads KV head h / G, G = H / Hk (the convention of `_ExpandKv` and decode_attn.cu).
+// With Hk == H every kernel does exactly what the multi-head kernels did.
+//
+// Layouts: q, dO [B, L, H, D=128] and k, v [B, L, Hk, D] bf16 views (strides (*, *, D, 1));
+// O [B, L, H, D] and dK, dV [B, L, Hk, D] contiguous bf16;  dq_part [Jc, B, L, H, D] fp32;
+// dk_part, dv_part [S, B, L, Hk, D] fp32 (only when the group is split, S > 1);  lse, delta
+// [B, H, L] fp32;  rel / drel [H, 2L-1] fp32;  segment ids / positions [B, L] int32 (optional).
 
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -123,6 +128,7 @@ struct FwdParams {
   __nv_bfloat16* out;    // [B, L, H, D]
   float* lse;            // [B, H, L] natural log
   int B, H, L;
+  int G;                 // query heads per KV head
   float scale;
 };
 
@@ -131,7 +137,8 @@ constexpr size_t kFwdSmem = kTile * 6 + 4096 + 1024;
 
 // K/V blocks stream through a two-stage TMA ring while each warpgroup runs
 //   S = Q·K^T (wgmma, registers) | online softmax | P (bf16) -> smem | O += P·V (wgmma)
-// on its 64 query rows.
+// on its 64 query rows. CTA = (query block, query head h, b); K/V come from KV head h / G.
+// The heads of a group are adjacent in blockIdx.y, so their K/V tiles are re-read from L2.
 __global__ void __launch_bounds__(kThreads, 1)
 flash_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                  const __grid_constant__ CUtensorMap map_v, const FwdParams p) {
@@ -185,8 +192,8 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
         mbar_wait(smem_u32(&kv_empty[s]), ((it >> 1) & 1) ^ 1);
         const uint32_t fb = smem_u32(&kv_full[s]);
         mbar_arrive_expect_tx(fb, 2 * kTile);
-        load_tile(s_kv + 2 * s * kTile, &map_k, fb, h, jb * kT, b);
-        load_tile(s_kv + (2 * s + 1) * kTile, &map_v, fb, h, jb * kT, b);
+        load_tile(s_kv + 2 * s * kTile, &map_k, fb, h / p.G, jb * kT, b);
+        load_tile(s_kv + (2 * s + 1) * kTile, &map_v, fb, h / p.G, jb * kT, b);
         ++it;
       }
     }
@@ -333,13 +340,22 @@ struct BwdParams {
   const float* lse;      // [B, H, L]
   const float* delta;    // [B, H, L]
   float* dq_part;        // [Jc, B, L, H, D] fp32: dQ of each key block of this launch
-  __nv_bfloat16* dk;     // [B, L, H, D]
-  __nv_bfloat16* dv;     // [B, L, H, D]
+  __nv_bfloat16* dk;     // [B, L, Hk, D] (S == 1)
+  __nv_bfloat16* dv;     // [B, L, Hk, D] (S == 1)
+  float* dk_part;        // [S, B, L, Hk, D] fp32 (S > 1, else nullptr)
+  float* dv_part;        // [S, B, L, Hk, D] fp32 (S > 1, else nullptr)
   float* drel_part;      // [B, H, Jc, 2L-1] fp32, zero-initialised (or nullptr)
   int B, H, L;
+  int Hk, G, S;          // KV heads, query heads per KV head, runs per group
   int j_begin, jc;       // this launch covers key blocks [j_begin, j_begin + jc)
   float scale;
 };
+
+// Key blocks per backward launch (the leading dimension of dq_part / drel_part).
+constexpr int kJChunk = 8;
+// The backward splits a group of query heads into S runs until one launch has at least this
+// many CTAs (about four per SM of an H100 SXM); see flash_attn_bwd_splits.
+constexpr int kBwdMinCtas = 512;
 
 constexpr int kBwdStages = 2;
 // K, V resident + 2 x (Q, dO) + one [128 keys x 64 queries] P/dS tile + barriers / tables.
@@ -351,6 +367,11 @@ constexpr size_t kBwdSmem = kTile * (2 + 2 * kBwdStages) + kChunk + 8192 + 1024;
 //   S^T = K·Q^T, dP^T = V·dO^T | P^T = exp2(S^T - lse), dS^T = P^T∘(dP^T - delta) |
 //   dV += P^T·dO | dK += dS^T·Q | dQ = dS·K -> this key block's slice of dq_part;
 //   d rel[h, i-j+L-1] += Σ dS along diagonals -> this CTA's row of drel_part.
+// Grouped KV heads: CTA = (key block, run r, b), where run r is the G/S query heads
+// [r·G/S, (r+1)·G/S) of KV head r / S. The CTA walks (query head, visible query block) in
+// that order and keeps dK, dV in registers over the whole run; lse, delta, the rel row and
+// the dq_part / drel_part rows belong to the query head. S == 1: dK, dV leave as bf16; S > 1:
+// as this run's slice of dk_part / dv_part, folded in run order by flash_dkv_fold_kernel.
 // No atomics: the partials are folded in key-block order by the reduce kernels below, so
 // the gradients are identical run to run.
 __global__ void __launch_bounds__(kThreads, 1)
@@ -360,7 +381,10 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
   const int nblk = p.L / kT;
   const int jrel = blockIdx.x;
   const int j_blk = p.j_begin + jrel;                         // key block (small j = long loop first)
-  const int h = blockIdx.y, b = blockIdx.z;
+  const int b = blockIdx.z;
+  const int nh = p.G / p.S;                                   // query heads of this CTA's run
+  const int h_first = blockIdx.y * nh;
+  const int hkv = h_first / p.G;
   const int j0 = j_blk * kT;
   const int4 kmeta = block_meta(p.mask, b, nblk, j_blk);
 
@@ -405,10 +429,11 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
     setmaxnreg_dec<40>();
     if (threadIdx.x == kConsumers) {
       mbar_arrive_expect_tx(smem_u32(kv_bar), 2 * kTile);
-      load_tile(s_k, &map_k, smem_u32(kv_bar), h, j0, b);
-      load_tile(s_v, &map_v, smem_u32(kv_bar), h, j0, b);
+      load_tile(s_k, &map_k, smem_u32(kv_bar), hkv, j0, b);
+      load_tile(s_v, &map_v, smem_u32(kv_bar), hkv, j0, b);
       int it = 0;
-      for (int ib = 0; ib < nblk; ++ib) {
+      for (int step = 0; step < nh * nblk; ++step) {   // (query head, query block) in order
+        const int h = h_first + step / nblk, ib = step % nblk;
         if (!pair_visible(p.mask, block_meta(p.mask, b, nblk, ib), kmeta)) continue;
         const int s = it % kBwdStages;
         mbar_wait(smem_u32(&empty_bar[s]), ((it / kBwdStages) & 1) ^ 1);
@@ -428,7 +453,6 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
   const int w16 = (warp_idx & 3) * 16 + (lane >> 2);       // fragment row (+ 8 i)
   const int cq = (lane & 3) * 2;
   const long long bl = static_cast<long long>(b) * p.L;
-  const long long bh = static_cast<long long>(b) * p.H + h;
   const float sl2 = p.scale * kLog2e;
   int segk[2], posk[2];
 #pragma unroll
@@ -443,9 +467,11 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
   mbar_wait(smem_u32(kv_bar), 0);
 
   int it = 0;
-  for (int ib = 0; ib < nblk; ++ib) {
+  for (int step = 0; step < nh * nblk; ++step) {     // (query head, query block) in order
+    const int h = h_first + step / nblk, ib = step % nblk;
     const int4 qmeta = block_meta(p.mask, b, nblk, ib);
     if (!pair_visible(p.mask, qmeta, kmeta)) continue;
+    const long long bh = static_cast<long long>(b) * p.H + h;
     const int i0 = ib * kT;
     const int s = it % kBwdStages;
     const bool full = pair_full(p.mask, qmeta, kmeta);
@@ -591,10 +617,24 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
     }
     ++it;
   }
-  // ---- dK, dV: registers → bf16 → global (row = key); zero when no query sees the block ----
+  // ---- dK, dV: registers → bf16 (or this run's fp32 partial) → global (row = key); zero
+  // when no query of the run sees the block ----
+  if (p.dk_part != nullptr) {
+    const long long part = static_cast<long long>(blockIdx.y % p.S) * p.B * p.L;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const long long orow = ((part + bl + j0 + wg * 64 + w16 + 8 * i) * p.Hk + hkv) * kD + cq;
+#pragma unroll
+      for (int n = 0; n < 16; ++n) {
+        *reinterpret_cast<float2*>(p.dv_part + orow + n * 8) = make_float2(dv[4 * n + 2 * i], dv[4 * n + 2 * i + 1]);
+        *reinterpret_cast<float2*>(p.dk_part + orow + n * 8) = make_float2(dk[4 * n + 2 * i], dk[4 * n + 2 * i + 1]);
+      }
+    }
+    return;
+  }
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    const long long orow = ((bl + j0 + wg * 64 + w16 + 8 * i) * p.H + h) * kD + cq;
+    const long long orow = ((bl + j0 + wg * 64 + w16 + 8 * i) * p.Hk + hkv) * kD + cq;
 #pragma unroll
     for (int n = 0; n < 16; ++n) {
       *reinterpret_cast<uint32_t*>(p.dv + orow + n * 8) =
@@ -699,12 +739,30 @@ flash_cast_kernel(const float4* __restrict__ src, uint2* __restrict__ dst, long 
   }
 }
 
-void CheckQkv(const torch::Tensor& t, const torch::Tensor& q, const char* name) {
+// dk, dv (bf16) = Σ_s dk_part[s], Σ_s dv_part[s] in fp32, in order of the run s.
+__global__ void __launch_bounds__(256)
+flash_dkv_fold_kernel(const float4* __restrict__ dk_part, const float4* __restrict__ dv_part,
+                      uint2* __restrict__ dk, uint2* __restrict__ dv, long long n4, int splits) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n4) return;
+  float4 a = dk_part[i], c = dv_part[i];
+  for (int s = 1; s < splits; ++s) {
+    const float4 x = dk_part[s * n4 + i], y = dv_part[s * n4 + i];
+    a.x += x.x; a.y += x.y; a.z += x.z; a.w += x.w;
+    c.x += y.x; c.y += y.y; c.z += y.z; c.w += y.w;
+  }
+  dk[i] = make_uint2(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w));
+  dv[i] = make_uint2(pack_bf16x2(c.x, c.y), pack_bf16x2(c.z, c.w));
+}
+
+// t is a bf16 view of shape `sizes` with strides (*, *, 128, 1) and 16-byte aligned rows.
+void CheckQkv(const char* op, const torch::Tensor& t, torch::IntArrayRef sizes, const char* name) {
   TORCH_CHECK(t.is_cuda() && t.scalar_type() == torch::kBFloat16 && t.dim() == 4 &&
-                  t.sizes() == q.sizes() && t.stride(3) == 1 && t.stride(2) == kD &&
+                  t.sizes() == sizes && t.stride(3) == 1 && t.stride(2) == kD &&
                   t.stride(1) % 8 == 0 && t.stride(0) % 8 == 0 &&
                   reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0,
-              "flash_attn: ", name, " must be a bf16 [B,L,H,128] view with strides (*, *, 128, 1)");
+              op, ": ", name, " must be a bf16 ", sizes,
+              " view with strides (*, *, 128, 1) and 16-byte aligned rows, got ", t.sizes());
 }
 
 bool Given(const c10::optional<torch::Tensor>& t) { return t.has_value() && t->defined(); }
@@ -715,8 +773,9 @@ const int* IntPtr(const c10::optional<torch::Tensor>& t) {
 
 // Argument checks of both entry points, made before anything is allocated or launched: every
 // tensor the kernels read or write is on q's device (a host `rel` would otherwise reach the
-// kernel as a host pointer), and seg / pos / lse have the shapes the kernels index. `out`,
-// `d_out` and `lse` are given by the backward only.
+// kernel as a host pointer), k and v are [B, L, Hk, 128] with H % Hk == 0, and rel / seg /
+// pos / out / d_out / lse have the shapes the kernels index. `out`, `d_out` and `lse` are
+// given by the backward only.
 void CheckArgs(const char* op, const torch::Tensor& q, const torch::Tensor& k,
                const torch::Tensor& v, const c10::optional<torch::Tensor>& rel,
                const c10::optional<torch::Tensor>& seg, const c10::optional<torch::Tensor>& pos,
@@ -730,11 +789,15 @@ void CheckArgs(const char* op, const torch::Tensor& q, const torch::Tensor& k,
     TORCH_CHECK(t.device() == q.device(), op, ": ", name, " is on ", t.device(),
                 " but q is on ", q.device());
   };
-  CheckQkv(q, q, "q");
+  CheckQkv(op, q, q.sizes(), "q");
   on_q(k, "k");
-  CheckQkv(k, q, "k");
+  TORCH_CHECK(k.dim() == 4 && k.size(0) == B && k.size(1) == L && k.size(2) >= 1 &&
+                  H % k.size(2) == 0 && k.size(3) == kD,
+              op, ": k must be [B, L, Hk, 128] with q's B and L and H % Hk == 0; q is ",
+              q.sizes(), ", k is ", k.sizes());
+  CheckQkv(op, k, k.sizes(), "k");
   on_q(v, "v");
-  CheckQkv(v, q, "v");
+  CheckQkv(op, v, k.sizes(), "v");
   if (Given(rel)) {
     on_q(*rel, "rel");
     TORCH_CHECK(rel->scalar_type() == torch::kFloat32 && rel->dim() == 2 && rel->size(0) == H &&
@@ -781,6 +844,20 @@ torch::Tensor BlockMeta(const int* seg, const int* pos, int64_t B, int64_t L,
 
 }  // namespace
 
+// Runs S into which the backward splits each group of G = H / Hk query heads: the smallest
+// divisor of G for which one key-block launch, min(L/128, kJChunk) x (Hk·S) x B CTAs, has at
+// least kBwdMinCtas CTAs (G when none has). It depends on the shapes only, so a problem is
+// split, and its dK / dV summed, the same way on every card. Always 1 for multi-head attention.
+int64_t flash_attn_bwd_splits(int64_t B, int64_t L, int64_t H, int64_t Hk) {
+  TORCH_CHECK(B >= 1 && L >= kT && Hk >= 1 && H % Hk == 0,
+              "flash_attn_bwd_splits: needs B >= 1, L >= 128 and H % Hk == 0");
+  const int64_t g = H / Hk;
+  const int64_t ctas = std::min<int64_t>(L / kT, kJChunk) * Hk * B;
+  int64_t s = 1;
+  while (s < g && (g % s != 0 || ctas * s < kBwdMinCtas)) ++s;
+  return s;
+}
+
 // Returns (out [B,L,H,D] bf16, lse [B,H,L] fp32).
 std::vector<torch::Tensor> flash_attn_fwd(const torch::Tensor& q, const torch::Tensor& k,
                                           const torch::Tensor& v,
@@ -808,9 +885,10 @@ std::vector<torch::Tensor> flash_attn_fwd(const torch::Tensor& q, const torch::T
   p.out = reinterpret_cast<__nv_bfloat16*>(out.data_ptr());
   p.lse = lse.data_ptr<float>();
   p.B = static_cast<int>(B); p.H = static_cast<int>(H); p.L = static_cast<int>(L);
+  p.G = static_cast<int>(H / k.size(2));
   p.scale = static_cast<float>(scale);
   auto mk = [&](const torch::Tensor& t) {
-    return MakeMap(t.data_ptr(), H * kD, L, B, t.stride(1), t.stride(0), kT);
+    return MakeMap(t.data_ptr(), t.size(2) * kD, L, B, t.stride(1), t.stride(0), kT);
   };
   const CUtensorMap mq = mk(q), mkk = mk(k), mv = mk(v);
   static bool configured = false;
@@ -826,7 +904,7 @@ std::vector<torch::Tensor> flash_attn_fwd(const torch::Tensor& q, const torch::T
   return {out, lse};
 }
 
-// Returns (dq, dk, dv [B,L,H,D] bf16, drel [H,2L-1] fp32 or an empty tensor).
+// Returns (dq [B,L,H,D], dk, dv [B,L,Hk,D] bf16, drel [H,2L-1] fp32 or an empty tensor).
 std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::Tensor& k,
                                           const torch::Tensor& v, const torch::Tensor& out,
                                           const torch::Tensor& d_out, const torch::Tensor& lse,
@@ -835,10 +913,11 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
                                           const c10::optional<torch::Tensor>& pos, double scale,
                                           bool causal, bool need_drel) {
   CheckArgs("flash_attn_bwd", q, k, v, rel, seg, pos, &out, &d_out, &lse);
-  const int64_t B = q.size(0), L = q.size(1), H = q.size(2);
+  const int64_t B = q.size(0), L = q.size(1), H = q.size(2), Hk = k.size(2);
+  const int64_t S = flash_attn_bwd_splits(B, L, H, Hk);
   const c10::cuda::CUDAGuard guard(q.device());
   auto d_o = d_out.contiguous();
-  CheckQkv(d_o, q, "dO");
+  CheckQkv("flash_attn_bwd", d_o, q.sizes(), "dO");
   auto stream = at::cuda::getCurrentCUDAStream();
   auto delta = torch::empty({B, H, L}, lse.options());
   {
@@ -868,16 +947,25 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
   auto blk = BlockMeta(p.mask.seg, p.mask.pos, B, L, q.options());
   p.mask.blk = blk.numel() ? reinterpret_cast<const int4*>(blk.data_ptr<int>()) : nullptr;
   auto dq_acc = torch::zeros({B, L, H, kD}, lse.options());
-  auto dk = torch::empty({B, L, H, kD}, q.options());
-  auto dv = torch::empty({B, L, H, kD}, q.options());
+  auto dk = torch::empty({B, L, Hk, kD}, q.options());
+  auto dv = torch::empty({B, L, Hk, kD}, q.options());
+  // S > 1: every CTA writes its key block's rows of its run's slice, so no zero-fill is needed.
+  torch::Tensor dk_part, dv_part;
+  if (S > 1) {
+    dk_part = torch::empty({S, B, L, Hk, kD}, lse.options());
+    dv_part = torch::empty({S, B, L, Hk, kD}, lse.options());
+  }
   p.lse = lse.data_ptr<float>();
   p.delta = delta.data_ptr<float>();
   p.dk = reinterpret_cast<__nv_bfloat16*>(dk.data_ptr());
   p.dv = reinterpret_cast<__nv_bfloat16*>(dv.data_ptr());
+  p.dk_part = S > 1 ? dk_part.data_ptr<float>() : nullptr;
+  p.dv_part = S > 1 ? dv_part.data_ptr<float>() : nullptr;
   p.B = static_cast<int>(B); p.H = static_cast<int>(H); p.L = static_cast<int>(L);
+  p.Hk = static_cast<int>(Hk); p.G = static_cast<int>(H / Hk); p.S = static_cast<int>(S);
   p.scale = static_cast<float>(scale);
   auto mk = [&](const torch::Tensor& t) {
-    return MakeMap(t.data_ptr(), H * kD, L, B, t.stride(1), t.stride(0), kT);
+    return MakeMap(t.data_ptr(), t.size(2) * kD, L, B, t.stride(1), t.stride(0), kT);
   };
   const CUtensorMap mq = mk(q), mkk = mk(k), mv = mk(v), mdo = mk(d_o);
   static bool configured = false;
@@ -888,7 +976,6 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
   }
   // Key blocks go in launches of up to kJChunk; each launch's per-key-block dQ / dRel partials
   // are folded in key-block order, so the result does not depend on CTA scheduling.
-  constexpr int kJChunk = 8;
   const int nblk = static_cast<int>(L / kT);
   const int jc_max = nblk < kJChunk ? nblk : kJChunk;
   auto dq_part = torch::empty({jc_max, B, L, H, kD}, lse.options());
@@ -903,7 +990,7 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
       drel_part = torch::zeros({B, H, jc, 2 * L - 1}, lse.options());
       p.drel_part = drel_part.data_ptr<float>();
     }
-    dim3 grid(static_cast<unsigned>(jc), static_cast<unsigned>(H), static_cast<unsigned>(B));
+    dim3 grid(static_cast<unsigned>(jc), static_cast<unsigned>(Hk * S), static_cast<unsigned>(B));
     flash_bwd_kernel<<<grid, kThreads, kBwdSmem, stream>>>(mq, mkk, mv, mdo, p);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
     const long long n4 = B * L * H * (kD / 4);
@@ -919,6 +1006,15 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
       C10_CUDA_KERNEL_LAUNCH_CHECK();
       CountLaunch();
     }
+  }
+  if (S > 1) {
+    const long long n4 = B * L * Hk * (kD / 4);
+    flash_dkv_fold_kernel<<<static_cast<int>((n4 + 255) / 256), 256, 0, stream>>>(
+        reinterpret_cast<const float4*>(p.dk_part), reinterpret_cast<const float4*>(p.dv_part),
+        reinterpret_cast<uint2*>(dk.data_ptr()), reinterpret_cast<uint2*>(dv.data_ptr()), n4,
+        p.S);
+    C10_CUDA_KERNEL_LAUNCH_CHECK();
+    CountLaunch();
   }
   auto dq = torch::empty({B, L, H, kD}, q.options());
   {
@@ -944,4 +1040,6 @@ LB_REGISTER(flash_attn) {
   m.def("flash_attn_bwd", &lb::flash_attn_bwd, py::arg("q"), py::arg("k"), py::arg("v"),
         py::arg("out"), py::arg("d_out"), py::arg("lse"), py::arg("rel"), py::arg("seg"),
         py::arg("pos"), py::arg("scale"), py::arg("causal"), py::arg("need_drel"));
+  m.def("flash_attn_bwd_splits", &lb::flash_attn_bwd_splits, py::arg("B"), py::arg("L"),
+        py::arg("H"), py::arg("Hk"));
 }

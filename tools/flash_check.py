@@ -4,6 +4,10 @@ Numerics against the fp32 oracle for forward, dQ/dK/dV and the bias-table gradie
 (several geometries: packed segments, padding, causal / bidirectional, with / without the
 relative bias), then timing at the benchmark shape. Writes the results as JSON and prints
 FLASH_OK.
+
+`--gqa` only times grouped-query / multi-query attention (`BenchGqa`): the flash kernels at
+Hk = H and Hk < H against the SDPA path that Hk < H took before. It prints one JSON line and,
+with `--out PATH`, also writes the result to PATH.
 """
 import json
 import os
@@ -12,6 +16,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
+from lingvo_b200 import ops
 from lingvo_b200.ops import attention as A
 
 
@@ -111,8 +116,62 @@ def Bench():
   return out
 
 
+def _FallbackCore(q, k, v, rel, seg, pos, causal):
+  """What `SelfAttentionLayer` ran for Hk < H before the kernels took grouped KV heads:
+  the bf16 [B, H, L, L] mask + Toeplitz bias, K/V expanded to H heads, SDPA."""
+  from lingvo_b200.core import gshard_builder
+  l = q.shape[1]
+  a, c = seg.unsqueeze(-1), seg.unsqueeze(-2)
+  not_vis = ((a == 0) & (c == 0)) | (a != c)
+  if causal:
+    not_vis = not_vis | (pos.unsqueeze(-1) < pos.unsqueeze(-2))
+  mask = (not_vis.to(q.dtype) * -1e9).unsqueeze(1)
+  bias = mask + A._RelToeplitz(rel, l).to(q.dtype).unsqueeze(0)
+  return gshard_builder._AttentionCore(q, k, v, bias)
+
+
+def BenchGqa():
+  """Forward and forward+backward times (us) of grouped / multi-query attention: the flash
+  kernels at Hk = H (multi-head, same FLOPs), Hk < H, and the SDPA path Hk < H took before,
+  at MoELm8E's shape (causal, relative bias) and at wiki_bert's (multi-query encoder)."""
+  dev = 'cuda'
+  res = {}
+  shapes = [('moe', 8, 1024, 16, (16, 4, 1), True), ('bert', 8, 512, 8, (8, 1), False)]
+  for name, b, l, h, hks, causal in shapes:
+    for hk in hks:
+      torch.manual_seed(0)
+      d = 128
+      q = (torch.randn(b, l, h, d, device=dev) * 0.5).bfloat16().requires_grad_(True)
+      k = (torch.randn(b, l, hk, d, device=dev) * 0.5).bfloat16().requires_grad_(True)
+      v = (torch.randn(b, l, hk, d, device=dev) * 0.5).bfloat16().requires_grad_(True)
+      rel = torch.randn(h, 2 * l - 1, device=dev).requires_grad_(True)
+      seg = torch.ones(b, l, dtype=torch.int32, device=dev)
+      pos = torch.arange(l, dtype=torch.int32, device=dev).unsqueeze(0).expand(b, l).contiguous()
+      d_o = (torch.randn(b, l, h, d, device=dev) * 0.5).bfloat16()
+      impls = {'flash': lambda: A.flash_attention(q, k, v, rel, seg, pos, 1.0, causal)}
+      if hk < h:
+        impls['sdpa'] = lambda: _FallbackCore(q, k, v, rel, seg, pos, causal)
+      for impl, fn in impls.items():
+        key = '%s_hk%d_%s' % (name, hk, impl)
+        with torch.no_grad():
+          res[key + '_fwd_us'] = Time(fn)
+        res[key + '_fwdbwd_us'] = Time(lambda: torch.autograd.grad(fn(), [q, k, v, rel], d_o))
+      if impls.get('sdpa'):
+        res['%s_hk%d_bwd_splits' % (name, hk)] = ops.native().flash_attn_bwd_splits(b, l, h, hk)
+  return res
+
+
 def main():
   assert torch.cuda.is_available()
+  if '--gqa' in sys.argv:               # timings of grouped / multi-query attention only
+    gqa = BenchGqa()
+    print(json.dumps(gqa))
+    if '--out' in sys.argv:
+      path = sys.argv[sys.argv.index('--out') + 1]
+      os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+      with open(path, 'w') as f:
+        json.dump(gqa, f, indent=1)
+    return
   results = []
   cases = [
       (1, 128, 1, False, 0, False, 1),
