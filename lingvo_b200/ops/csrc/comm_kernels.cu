@@ -9,8 +9,6 @@
 //       ONE kernel: shard gradients are summed from the peers, the fp32 master
 //       shard and its Adam moments are updated, and the new bf16 weights are
 //       stored straight into every peer's replica of the parameters.
-//   tp_reduce_slabs : owner-side sum of the W partial slabs written by the
-//       row-pointer epilogue of the tensor-parallel GEMM (GEMM -> reduce-scatter).
 // The device-counter flags of moe_sync order the phases across ranks.
 
 #include <ATen/cuda/CUDAContext.h>
@@ -125,48 +123,6 @@ zero_adam_kernel(const PeerPtrs grads, const PeerPtrs params, float* __restrict_
   }
 }
 
-// out[row, :] = sum_w slabs[w, row, :]   (bf16 in, bf16 out, fp32 accumulate)
-__global__ void tp_reduce_slabs_kernel(const __nv_bfloat16* __restrict__ slabs,
-                                       __nv_bfloat16* __restrict__ out, long long n8, int world) {
-  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n8;
-       i += stride) {
-    float a[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int w = 0; w < world; ++w)
-      acc8(a, *(reinterpret_cast<const int4*>(slabs) + static_cast<long long>(w) * n8 + i));
-    int4 o;
-    o.x = pack_bf16x2(a[0], a[1]);
-    o.y = pack_bf16x2(a[2], a[3]);
-    o.z = pack_bf16x2(a[4], a[5]);
-    o.w = pack_bf16x2(a[6], a[7]);
-    *(reinterpret_cast<int4*>(out) + i) = o;
-  }
-}
-
-// Same sum, but the reduced [rows, cols] block is stored at column offset
-// `col_off` of a [rows, out_ld] matrix on every peer (reduce-scatter + all-gather
-// = all-reduce, with the gather done by NVLink stores from the reducing rank).
-__global__ void tp_reduce_bcast_kernel(const __nv_bfloat16* __restrict__ slabs, const PeerPtrs outs,
-                                       int n_out, long long rows, int cols8, long long out_ld8,
-                                       int col_off8, int world) {
-  const long long n8 = rows * cols8;
-  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n8;
-       i += stride) {
-    float a[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int w = 0; w < world; ++w)
-      acc8(a, *(reinterpret_cast<const int4*>(slabs) + static_cast<long long>(w) * n8 + i));
-    int4 o;
-    o.x = pack_bf16x2(a[0], a[1]);
-    o.y = pack_bf16x2(a[2], a[3]);
-    o.z = pack_bf16x2(a[4], a[5]);
-    o.w = pack_bf16x2(a[6], a[7]);
-    const long long r = i / cols8;
-    const long long dst = r * out_ld8 + col_off8 + (i - r * cols8);
-    for (int q = 0; q < n_out; ++q) *(reinterpret_cast<int4*>(outs.p[q]) + dst) = o;
-  }
-}
-
 PeerPtrs ToPeers(const torch::Tensor& t) {
   TORCH_CHECK(t.device().is_cpu() && t.scalar_type() == torch::kInt64 && t.numel() <= kMaxWorld,
               "peer pointer table must be a CPU int64 tensor of <= 16 entries");
@@ -222,47 +178,13 @@ void zero_adam(const torch::Tensor& grad_peers_cpu, const torch::Tensor& param_p
   CountLaunch();
 }
 
-torch::Tensor tp_reduce_slabs(const torch::Tensor& slabs, int64_t world) {
-  TORCH_CHECK(slabs.is_cuda() && slabs.scalar_type() == torch::kBFloat16 && slabs.is_contiguous());
-  TORCH_CHECK(slabs.size(0) == world && (slabs.numel() / world) % 8 == 0);
-  const c10::cuda::CUDAGuard guard(slabs.device());
-  auto sizes = slabs.sizes().vec();
-  sizes.erase(sizes.begin());
-  auto out = torch::empty(sizes, slabs.options());
-  const long long n8 = out.numel() / 8;
-  tp_reduce_slabs_kernel<<<Blocks(n8), 512, 0, at::cuda::getCurrentCUDAStream()>>>(
-      reinterpret_cast<const __nv_bfloat16*>(slabs.data_ptr()),
-      reinterpret_cast<__nv_bfloat16*>(out.data_ptr()), n8, (int)world);
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
-  CountLaunch();
-  return out;
-}
-
-void tp_reduce_bcast(const torch::Tensor& slabs, int64_t world, const torch::Tensor& out_ptrs_cpu,
-                     int64_t out_ld, int64_t col_off) {
-  TORCH_CHECK(slabs.is_cuda() && slabs.scalar_type() == torch::kBFloat16 && slabs.is_contiguous() &&
-              slabs.dim() == 3 && slabs.size(0) == world);
-  const int64_t rows = slabs.size(1), cols = slabs.size(2);
-  TORCH_CHECK(cols % 8 == 0 && out_ld % 8 == 0 && col_off % 8 == 0);
-  const c10::cuda::CUDAGuard guard(slabs.device());
-  const long long n8 = rows * cols / 8;
-  tp_reduce_bcast_kernel<<<Blocks(n8), 512, 0, at::cuda::getCurrentCUDAStream()>>>(
-      reinterpret_cast<const __nv_bfloat16*>(slabs.data_ptr()), ToPeers(out_ptrs_cpu),
-      static_cast<int>(out_ptrs_cpu.numel()), rows, static_cast<int>(cols / 8), out_ld / 8,
-      static_cast<int>(col_off / 8), static_cast<int>(world));
-  C10_CUDA_KERNEL_LAUNCH_CHECK();
-  CountLaunch();
-}
-
 }  // namespace lb
 
 LB_REGISTER(comm) {
-  m.def("tp_reduce_bcast", &lb::tp_reduce_bcast);
   m.attr("_has_comm") = true;
   m.def("allreduce_mean_bf16", &lb::allreduce_mean_bf16, pybind11::arg("peer_ptrs_cpu"),
         pybind11::arg("shard_elems"), pybind11::arg("rank"), pybind11::arg("world"),
         pybind11::arg("scale"), pybind11::arg("device"), pybind11::arg("store_all"),
         pybind11::arg("sumsq"), pybind11::arg("max_blocks") = 0);
   m.def("zero_adam", &lb::zero_adam);
-  m.def("tp_reduce_slabs", &lb::tp_reduce_slabs);
 }

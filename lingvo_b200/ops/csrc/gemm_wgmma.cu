@@ -15,20 +15,22 @@
 //   groups in a fixed order (bands of kGroupM M-tiles, for L2 reuse), and the
 //   producer runs ahead across tile boundaries, so the ring refills for the next
 //   tile while the consumers run this tile's epilogue;
-// * plain bf16 outputs leave by TMA: each consumer warpgroup applies the fused
-//   epilogue (bias, activation, ReLU-gradient mask / residual add, per-row scale)
-//   in its accumulator layout, writes bf16 into a 64 x 64 swizzled staging slice
-//   and one thread issues a bulk tensor store, so the next tile's MMAs start
-//   without waiting for global memory. The residual / ReLU-mask operand arrives
-//   the same way: TMA loads it into the staging slice ahead of use and the
-//   epilogue overwrites it in place. The epilogue kinds the models use are
-//   compiled as separate specialisations, picked once per tile;
-// * the general epilogue (also accumulate into fp32, pre-activation tap, and
-//   redirected rows) stages fp32 accumulators through shared memory, 64 columns at
-//   a time, and then works on 8 adjacent columns of a row per thread, so every
-//   global load and store is a 16-byte row-contiguous vector. The store target of
-//   every output row can be redirected through a row-pointer table, which is how
-//   the MoE combine (expert GEMM -> NVLink peer store) is fused.
+// * the output is bf16. The fused epilogue is bias, then ReLU or nothing, then a
+//   ReLU-gradient mask or a residual add (never both, and neither after ReLU),
+//   then a per-row scale;
+// * outputs leave by TMA: each consumer warpgroup applies the epilogue in its
+//   accumulator layout, writes bf16 into a 64 x 64 swizzled staging slice and one
+//   thread issues a bulk tensor store, so the next tile's MMAs start without
+//   waiting for global memory. The residual / ReLU-mask operand arrives the same
+//   way: TMA loads it into the staging slice ahead of use and the epilogue
+//   overwrites it in place. The four epilogue kinds (plain, ReLU, residual add,
+//   ReLU mask) are compiled as separate specialisations, picked once per tile;
+// * the general epilogue serves redirected rows only: the store target of every
+//   output row comes from a row-pointer table, which is how the MoE combine
+//   (expert GEMM -> NVLink peer store) is fused. It stages fp32 accumulators
+//   through shared memory, 64 columns at a time, and then works on 8 adjacent
+//   columns of a row per thread, so every global load and store is a 16-byte
+//   row-contiguous vector.
 //
 // Every output tile is computed by one CTA with the same k-block order and wgmma
 // shape as a one-tile-per-CTA launch, so results do not depend on the grid size.
@@ -59,74 +61,52 @@ constexpr int kNumThreads = kNumConsumers + 128;   // + the TMA producer warpgro
 constexpr int kEpiCols = 64;  // columns per epilogue staging slice
 constexpr int kGroupM = 8;    // M-tiles per rasterisation band
 
-enum Act : int { kActNone = 0, kActRelu = 1, kActGelu = 2, kActSilu = 3, kActGeluTanh = 4,
-                 kActSquaredRelu = 5 };
+enum Act : int { kActNone = 0, kActRelu = 1 };
 enum AuxMode : int { kAuxNone = 0, kAuxReluMask = 1, kAuxAdd = 2 };
 // Epilogue specialisations of the TMA-store path (bias and row scale are uniform branches
-// inside each); kEpiGeneric reads the activation and aux mode from GemmParams.
-enum EpiKind : int { kEpiPlain = 0, kEpiRelu = 1, kEpiAdd = 2, kEpiMask = 3, kEpiGeneric = 4 };
-
-// A operand may be split along K over several tensor maps (one per NVLink peer):
-// the TMA producer then *is* the all-gather (tiles are pulled straight from the
-// owning rank's memory), SURVEY K5/K6 "all-gather -> GEMM".
-constexpr int kMaxAMaps = 8;
-struct TmapArray {
-  CUtensorMap m[kMaxAMaps];
-};
+// inside each).
+enum EpiKind : int { kEpiPlain = 0, kEpiRelu = 1, kEpiAdd = 2, kEpiMask = 3 };
 
 struct GemmParams {
   int G, M, N, K;
-  void* c;                 // [G, M, N] out (bf16 or fp32)
   long long ldc;           // row stride of C (elements)
   long long c_batch;       // batch stride of C (elements)
   const float* bias;       // [G, N] fp32 or nullptr
   const __nv_bfloat16* aux;  // [G, M, N] bf16 (same strides as C) or nullptr
-  void* pre_act;           // optional second output: pre-activation (bf16), same strides
   const float* row_scale;  // [G, M] or nullptr
   void* const* row_ptrs;   // [G * M] destination row pointers (peer memory) or nullptr
-  void* const* nblk_ptrs;  // [tiles_n] destination base per N-tile (peer slab) or nullptr;
-                           // element (row, col) goes to base[n_blk] + row*ldc + (col - n0)
-  int a_k_per_map;         // K elements covered by each A tensor map (all-gather prologue)
   int act;
   int aux_mode;
-  int accumulate;          // C += result (fp32 out only)
   int epi;                 // EpiKind (TMA-store path only)
 };
 
-__device__ __forceinline__ float apply_act(float x, int act) {
-  switch (act) {
-    case kActRelu: return fmaxf(x, 0.f);
-    case kActGelu: return 0.5f * x * (1.f + erff(x * 0.70710678118654752f));
-    case kActSilu: return x / (1.f + __expf(-x));
-    case kActGeluTanh: {
-      float u = 0.7978845608028654f * (x + 0.044715f * x * x * x);
-      return 0.5f * x * (1.f + tanhf(u));
-    }
-    case kActSquaredRelu: { float r = fmaxf(x, 0.f); return r * r; }
-    default: return x;
-  }
+// The fused epilogue of one output element, shared by both epilogues so that they round
+// alike: + bias b, activation, ReLU-gradient mask or residual add with the aux element x,
+// times the row scale rs. b and rs are read only when p has a bias / row scale.
+__device__ __forceinline__ float epilogue_elem(const GemmParams& p, float v, float b, int act,
+                                               int aux_mode, float x, float rs) {
+  if (p.bias != nullptr) v += b;
+  if (act == kActRelu) v = fmaxf(v, 0.f);
+  if (aux_mode == kAuxReluMask) v = x > 0.f ? v : 0.f;
+  else if (aux_mode == kAuxAdd) v += x;
+  if (p.row_scale != nullptr) v *= rs;
+  return v;
 }
 
-// Eight adjacent output columns of one row, read row-contiguously from the staging buffer:
-// bias / pre-act tap / activation / aux (ReLU-mask or residual add) / row scale / convert /
-// store. `off` is the element offset of (row, col) in the C-shaped aux / pre_act tensors,
-// `dst` the destination of (row, col); all of them are 16-byte aligned.
-template <typename OutT>
-__device__ __forceinline__ void epilogue_vec8(const GemmParams& p, float (&v)[8], OutT* dst,
-                                              long long off, const float* bias, float rscale) {
+// Eight adjacent output columns of one row, read row-contiguously from the staging buffer,
+// through epilogue_elem to the bf16 row at `dst`. `off` is the element offset of (row, col) in
+// the C-shaped aux tensor; both are 16-byte aligned.
+__device__ __forceinline__ void epilogue_vec8(const GemmParams& p, float (&v)[8],
+                                              __nv_bfloat16* dst, long long off,
+                                              const float* bias, float rscale) {
+  float b[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   if (bias != nullptr) {
     const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias));
     const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias) + 1);
-    v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w;
-    v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;
+    b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w;
+    b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
   }
-  if (p.pre_act != nullptr) {
-    const int4 o = make_int4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]),
-                             pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-    *reinterpret_cast<int4*>(reinterpret_cast<__nv_bfloat16*>(p.pre_act) + off) = o;
-  }
-#pragma unroll
-  for (int j = 0; j < 8; ++j) v[j] = apply_act(v[j], p.act);
+  float x[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   if (p.aux_mode != kAuxNone) {
     const int4 raw = *reinterpret_cast<const int4*>(p.aux + off);
     const uint32_t w[4] = {static_cast<uint32_t>(raw.x), static_cast<uint32_t>(raw.y),
@@ -134,32 +114,14 @@ __device__ __forceinline__ void epilogue_vec8(const GemmParams& p, float (&v)[8]
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 t = unpack_bf16x2(w[j]);
-      if (p.aux_mode == kAuxReluMask) {
-        v[2 * j] = t.x > 0.f ? v[2 * j] : 0.f;
-        v[2 * j + 1] = t.y > 0.f ? v[2 * j + 1] : 0.f;
-      } else {
-        v[2 * j] += t.x;
-        v[2 * j + 1] += t.y;
-      }
+      x[2 * j] = t.x;
+      x[2 * j + 1] = t.y;
     }
   }
 #pragma unroll
-  for (int j = 0; j < 8; ++j) v[j] *= rscale;
-  if constexpr (sizeof(OutT) == 2) {
-    *reinterpret_cast<int4*>(dst) = make_int4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]),
-                                              pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-  } else {
-    float4* out = reinterpret_cast<float4*>(dst);
-    float4 o0 = make_float4(v[0], v[1], v[2], v[3]);
-    float4 o1 = make_float4(v[4], v[5], v[6], v[7]);
-    if (p.accumulate) {
-      const float4 a0 = out[0], a1 = out[1];
-      o0.x += a0.x; o0.y += a0.y; o0.z += a0.z; o0.w += a0.w;
-      o1.x += a1.x; o1.y += a1.y; o1.z += a1.z; o1.w += a1.w;
-    }
-    out[0] = o0;
-    out[1] = o1;
-  }
+  for (int j = 0; j < 8; ++j) v[j] = epilogue_elem(p, v[j], b[j], p.act, p.aux_mode, x[j], rscale);
+  *reinterpret_cast<int4*>(dst) = make_int4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]),
+                                            pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
 }
 
 template <int BN, bool kAK, bool kBK>
@@ -213,15 +175,12 @@ __device__ __forceinline__ uint32_t staging_off(int r, int u) {
 // 64 columns alternate between the warpgroup's two bf16 staging buffers (`stg`, 128-byte
 // swizzled rows, the layout of the output / aux tensor maps). The first aux slice was loaded
 // during the MMA loop; the next one is loaded as soon as its buffer's store has read it.
-// Per element the arithmetic is that of epilogue_vec8. kAct / kAux < 0: read from p.
 template <int BN, int kAct, int kAux>
 __device__ __forceinline__ void epilogue_tma(const GemmParams& p, float (&acc)[BN / 2],
                                              const CUtensorMap* tmap_c,
                                              const CUtensorMap* tmap_aux, uint32_t stg,
                                              uint32_t aux_bar, uint32_t& aux_par, int row0,
                                              int n0, int g, int wg) {
-  const int act = kAct >= 0 ? kAct : p.act;
-  const int aux_mode = kAux >= 0 ? kAux : p.aux_mode;
   const int t = threadIdx.x & 127;
   const bool leader = t == 0;
   const int r = (t >> 5) * 16 + ((t & 31) >> 2);   // fragment rows r and r + 8
@@ -239,7 +198,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmParams& p, float (&acc)[B
     const int c0 = n0 + s * kEpiCols;
     if (c0 >= p.N) break;
     const uint32_t buf = stg + (s & 1) * kSliceBytes;
-    if (aux_mode != kAuxNone) {
+    if (kAux != kAuxNone) {
       mbar_wait(aux_bar + (s & 1) * 8, (aux_par >> (s & 1)) & 1);
       aux_par ^= 1u << (s & 1);
     } else {
@@ -255,23 +214,14 @@ __device__ __forceinline__ void epilogue_tma(const GemmParams& p, float (&acc)[B
       for (int i = 0; i < 2; ++i) {
         const uint32_t addr = buf + (r + 8 * i) * 128 + ((n ^ (r & 7)) << 4) + q * 4;
         const int a = 4 * (s * (kEpiCols / 8) + n) + 2 * i;
-        float v0 = acc[a], v1 = acc[a + 1];
-        if (bias != nullptr) { v0 += b.x; v1 += b.y; }
-        v0 = apply_act(v0, act);
-        v1 = apply_act(v1, act);
-        if (aux_mode != kAuxNone) {
+        float2 x = make_float2(0.f, 0.f);
+        if (kAux != kAuxNone) {
           uint32_t w;
           asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(addr) : "memory");
-          const float2 x = unpack_bf16x2(w);
-          if (aux_mode == kAuxReluMask) {
-            v0 = x.x > 0.f ? v0 : 0.f;
-            v1 = x.y > 0.f ? v1 : 0.f;
-          } else {
-            v0 += x.x;
-            v1 += x.y;
-          }
+          x = unpack_bf16x2(w);
         }
-        if (p.row_scale != nullptr) { v0 *= rs[i]; v1 *= rs[i]; }
+        const float v0 = epilogue_elem(p, acc[a], b.x, kAct, kAux, x.x, rs[i]);
+        const float v1 = epilogue_elem(p, acc[a + 1], b.y, kAct, kAux, x.y, rs[i]);
         asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_bf16x2(v0, v1)) : "memory");
       }
     }
@@ -280,7 +230,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmParams& p, float (&acc)[B
     if (leader) {
       tma_store_3d(tmap_c, buf, c0, row0, g);
       tma_store_commit();
-      if (aux_mode != kAuxNone && s + 1 < BN / kEpiCols && c0 + kEpiCols < p.N) {
+      if (kAux != kAuxNone && s + 1 < BN / kEpiCols && c0 + kEpiCols < p.N) {
         tma_store_wait_read<1>();   // slice s - 1 has left the other buffer
         const uint32_t nb = aux_bar + ((s + 1) & 1) * 8;
         mbar_arrive_expect_tx(nb, kSliceBytes);
@@ -290,17 +240,16 @@ __device__ __forceinline__ void epilogue_tma(const GemmParams& p, float (&acc)[B
   }
 }
 
-// kTmaStore: bf16 out through tmap_c (and aux through tmap_aux); otherwise the general
-// epilogue, which ignores both maps.
-template <int BN, bool kAK, bool kBK, typename OutT, bool kTmaStore>
+// kTmaStore: out through tmap_c (and aux through tmap_aux); otherwise the general epilogue,
+// which stores through p.row_ptrs and ignores both maps.
+template <int BN, bool kAK, bool kBK, bool kTmaStore>
 __global__ void __launch_bounds__(kNumThreads, 1)
-gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
                   const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_c,
                   const __grid_constant__ CUtensorMap tmap_aux, const GemmParams p) {
   using TS = TileShape<BN>;
   constexpr int kStages = TS::kStages;
-  static_assert(!kTmaStore || sizeof(OutT) == 2, "TMA-store epilogue writes bf16");
   static_assert(2 * kSliceBytes <= TS::kStagingBytes / 2, "two bf16 slices per warpgroup");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -322,7 +271,7 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
   const int num_k_blocks = (p.K + kBlockK - 1) / kBlockK;
 
   if (threadIdx.x == kNumConsumers) {
-    tma_prefetch_desc(&tmaps_a.m[0]);
+    tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     if constexpr (kTmaStore) {
       tma_prefetch_desc(&tmap_c);
@@ -355,14 +304,12 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
           const uint32_t sa = smem_u32(smem + stage * TS::kStageBytes);
           const uint32_t sb = sa + TS::kABytes;
           const int k0 = kb * kBlockK;
-          const int amap = k0 / p.a_k_per_map;
-          const int ka = k0 - amap * p.a_k_per_map;
           if constexpr (kAK) {
-            tma_load_3d(sa, &tmaps_a.m[amap], fb, ka, m0, g);
+            tma_load_3d(sa, &tmap_a, fb, k0, m0, g);
           } else {
 #pragma unroll
             for (int i = 0; i < kBlockM / 64; ++i)
-              tma_load_3d(sa + i * (64 * kBlockK * 2), &tmaps_a.m[amap], fb, m0 + 64 * i, ka, g);
+              tma_load_3d(sa + i * (64 * kBlockK * 2), &tmap_a, fb, m0 + 64 * i, k0, g);
           }
           if constexpr (kBK) {
             tma_load_3d(sb, &tmap_b, fb, k0, n0, g);
@@ -462,15 +409,12 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
             epilogue_tma<BN, kActNone, kAuxReluMask>(p, acc, &tmap_c, &tmap_aux, stg, aux_bar,
                                                      aux_par, row0, n0, g, wg);
             break;
-          default:
-            epilogue_tma<BN, -1, -1>(p, acc, &tmap_c, &tmap_aux, stg, aux_bar, aux_par, row0,
-                                     n0, g, wg);
         }
       }
       continue;
     }
 
-    // ======================== general epilogue ========================
+    // ================= general epilogue (redirected rows) =================
     // Per 64-column slice: fragments -> staging (fp32), then each thread takes 8 adjacent
     // columns of a row, so every global access is a 16-byte row-contiguous vector.
     const int frow = (warp_idx & 3) * 16 + (lane >> 2);
@@ -499,20 +443,11 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
         const int r = rsub + 16 * pass;
         const int row = m0 + wg * 64 + r;
         if (row >= p.M || col >= p.N) continue;
-        OutT* dst;
+        __nv_bfloat16* dst =
+            reinterpret_cast<__nv_bfloat16*>(p.row_ptrs[static_cast<long long>(g) * p.M + row]);
+        if (dst == nullptr) continue;
         const long long row_off =
             static_cast<long long>(g) * p.c_batch + static_cast<long long>(row) * p.ldc;
-        if (p.row_ptrs != nullptr) {
-          dst = reinterpret_cast<OutT*>(p.row_ptrs[static_cast<long long>(g) * p.M + row]);
-          if (dst == nullptr) continue;
-          dst += col;
-        } else if (p.nblk_ptrs != nullptr) {
-          // one destination slab per 256 output columns
-          dst = reinterpret_cast<OutT*>(p.nblk_ptrs[col >> 8]) +
-                static_cast<long long>(row) * p.ldc + (col & 255);
-        } else {
-          dst = reinterpret_cast<OutT*>(p.c) + row_off + col;
-        }
         float4 h0, h1;
         asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
                      : "=f"(h0.x), "=f"(h0.y), "=f"(h0.z), "=f"(h0.w)
@@ -525,7 +460,7 @@ gemm_wgmma_kernel(const __grid_constant__ TmapArray tmaps_a,
         const float rscale =
             p.row_scale != nullptr ? p.row_scale[static_cast<long long>(g) * p.M + row] : 1.f;
         const float* bias = p.bias ? p.bias + static_cast<long long>(g) * p.N + col : nullptr;
-        epilogue_vec8<OutT>(p, v, dst, row_off + col, bias, rscale);
+        epilogue_vec8(p, v, dst + col, row_off + col, bias, rscale);
       }
     }
   }
@@ -587,12 +522,12 @@ CUtensorMap MakeMap(const void* base, int64_t inner, int64_t rows, int64_t group
   return m;
 }
 
-template <int BN, bool kAK, bool kBK, typename OutT, bool kTmaStore>
-static void Launch(const TmapArray& ta, const CUtensorMap& tb, const CUtensorMap& tc,
+template <int BN, bool kAK, bool kBK, bool kTmaStore>
+static void Launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
                    const CUtensorMap& tx, const GemmParams& p, int sms, cudaStream_t stream) {
   constexpr size_t smem = TileShape<BN>::kSmemBytes;
   static_assert(smem <= 227 * 1024, "GEMM shared memory exceeds the sm_90 limit");
-  auto kern = gemm_wgmma_kernel<BN, kAK, kBK, OutT, kTmaStore>;
+  auto kern = gemm_wgmma_kernel<BN, kAK, kBK, kTmaStore>;
   static bool configured = false;
   if (!configured) {
     C10_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -608,14 +543,14 @@ static void Launch(const TmapArray& ta, const CUtensorMap& tb, const CUtensorMap
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
-template <int BN, typename OutT, bool kTmaStore>
-static void Dispatch(bool ak, bool bk, const TmapArray& ta, const CUtensorMap& tb,
+template <int BN, bool kTmaStore>
+static void Dispatch(bool ak, bool bk, const CUtensorMap& ta, const CUtensorMap& tb,
                      const CUtensorMap& tc, const CUtensorMap& tx, const GemmParams& p, int sms,
                      cudaStream_t s) {
-  if (ak && bk) Launch<BN, true, true, OutT, kTmaStore>(ta, tb, tc, tx, p, sms, s);
-  else if (ak && !bk) Launch<BN, true, false, OutT, kTmaStore>(ta, tb, tc, tx, p, sms, s);
-  else if (!ak && bk) Launch<BN, false, true, OutT, kTmaStore>(ta, tb, tc, tx, p, sms, s);
-  else Launch<BN, false, false, OutT, kTmaStore>(ta, tb, tc, tx, p, sms, s);
+  if (ak && bk) Launch<BN, true, true, kTmaStore>(ta, tb, tc, tx, p, sms, s);
+  else if (ak && !bk) Launch<BN, true, false, kTmaStore>(ta, tb, tc, tx, p, sms, s);
+  else if (!ak && bk) Launch<BN, false, true, kTmaStore>(ta, tb, tc, tx, p, sms, s);
+  else Launch<BN, false, false, kTmaStore>(ta, tb, tc, tx, p, sms, s);
 }
 
 // Tile width from the shape: 256 unless N is small, or unless 128-wide tiles finish at
@@ -631,19 +566,23 @@ static bool UseBn256(int64_t G, int64_t M, int64_t N, int sms) {
 }
 
 // a: [G, M, K] if a_kmajor else [G, K, M];  b: [G, N, K] if b_kmajor else [G, K, N]
-// (2-D inputs are treated as G = 1).  Returns / fills out [G, M, N].
+// (2-D inputs are treated as G = 1).  Returns / fills the bf16 out [G, M, N]; with row_ptrs,
+// row (g, m) goes to row_ptrs[g * M + m] instead (skipped where that is 0).
 torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bool a_kmajor,
                         bool b_kmajor, const c10::optional<torch::Tensor>& bias,
                         int64_t act, const c10::optional<torch::Tensor>& aux, int64_t aux_mode,
                         const c10::optional<torch::Tensor>& row_scale,
-                        const c10::optional<torch::Tensor>& out_opt, bool out_fp32,
-                        bool accumulate, const c10::optional<torch::Tensor>& pre_act,
-                        const c10::optional<torch::Tensor>& row_ptrs,
-                        const c10::optional<torch::Tensor>& nblk_ptrs,
-                        const c10::optional<torch::Tensor>& a_peer_ptrs, int64_t nblk_ld) {
+                        const c10::optional<torch::Tensor>& out_opt,
+                        const c10::optional<torch::Tensor>& row_ptrs) {
   TORCH_CHECK(a_in.is_cuda() && b_in.is_cuda(), "gemm_bf16: CUDA tensors required");
   TORCH_CHECK(a_in.scalar_type() == torch::kBFloat16 && b_in.scalar_type() == torch::kBFloat16,
               "gemm_bf16: bf16 inputs required");
+  const bool has_aux = aux.has_value() && aux->defined() && aux_mode != kAuxNone;
+  TORCH_CHECK(act == kActNone || act == kActRelu,
+              "gemm_bf16: act must be 0 (none) or 1 (ReLU), got ", act);
+  TORCH_CHECK(aux_mode >= kAuxNone && aux_mode <= kAuxAdd,
+              "gemm_bf16: aux_mode must be 0 (none), 1 (ReLU mask) or 2 (add), got ", aux_mode);
+  TORCH_CHECK(act == kActNone || !has_aux, "gemm_bf16: ReLU does not combine with an aux operand");
   const c10::cuda::CUDAGuard guard(a_in.device());
   torch::Tensor a = a_in.dim() == 2 ? a_in.unsqueeze(0) : a_in;
   torch::Tensor b = b_in.dim() == 2 ? b_in.unsqueeze(0) : b_in;
@@ -656,8 +595,7 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
   const int64_t K = a_kmajor ? a.size(2) : a.size(1);
   const int64_t N = b_kmajor ? b.size(1) : b.size(2);
   const int64_t Kb = b_kmajor ? b.size(2) : b.size(1);
-  const bool ag_prologue = a_peer_ptrs.has_value() && a_peer_ptrs->defined();
-  TORCH_CHECK(ag_prologue || K == Kb, "gemm_bf16: K mismatch ", K, " vs ", Kb);
+  TORCH_CHECK(K == Kb, "gemm_bf16: K mismatch ", K, " vs ", Kb);
   TORCH_CHECK(N % 8 == 0, "gemm_bf16: N must be a multiple of 8");
   auto check_op = [](const torch::Tensor& t) {
     TORCH_CHECK(t.stride(1) % 8 == 0 && (t.size(0) == 1 || t.stride(0) % 8 == 0) &&
@@ -672,32 +610,25 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
     out = out_opt.value();
     TORCH_CHECK(out.stride(-1) == 1, "gemm_bf16: out must be row-contiguous");
   } else {
-    out = torch::empty({G, M, N}, a.options().dtype(out_fp32 ? torch::kFloat32 : torch::kBFloat16));
+    out = torch::empty({G, M, N}, a.options());
   }
-  const bool fp32 = out.scalar_type() == torch::kFloat32;
-  TORCH_CHECK(fp32 || out.scalar_type() == torch::kBFloat16, "gemm_bf16: out dtype");
+  TORCH_CHECK(out.scalar_type() == torch::kBFloat16, "gemm_bf16: out must be bf16");
   torch::Tensor out3 = out.dim() == 2 ? out.unsqueeze(0) : out;
   TORCH_CHECK(out3.size(0) == G && out3.size(1) == M && out3.size(2) == N, "gemm_bf16: out shape");
 
   // The epilogue moves 8 columns per 16-byte access (row_ptrs rows must be 16-byte aligned
   // as well).
   auto aligned16 = [](const void* ptr) { return reinterpret_cast<uintptr_t>(ptr) % 16 == 0; };
-  const int64_t vec = fp32 ? 4 : 8;
-  TORCH_CHECK(aligned16(out3.data_ptr()) && out3.stride(1) % vec == 0 &&
-                  (G == 1 || out3.stride(0) % vec == 0),
+  TORCH_CHECK(aligned16(out3.data_ptr()) && out3.stride(1) % 8 == 0 &&
+                  (G == 1 || out3.stride(0) % 8 == 0),
               "gemm_bf16: out rows must be 16-byte aligned");
 
   GemmParams p;
   p.G = static_cast<int>(G); p.M = static_cast<int>(M); p.N = static_cast<int>(N);
   p.K = static_cast<int>(K);
-  p.c = out3.data_ptr();
   p.ldc = out3.stride(1);
   p.c_batch = G > 1 ? out3.stride(0) : 0;
-  p.bias = nullptr; p.aux = nullptr; p.row_scale = nullptr; p.pre_act = nullptr;
-  p.row_ptrs = nullptr;
-  p.nblk_ptrs = nullptr;
-  p.epi = kEpiGeneric;
-  p.a_k_per_map = static_cast<int>(K);
+  p.bias = nullptr; p.aux = nullptr; p.row_scale = nullptr; p.row_ptrs = nullptr;
   torch::Tensor bias_f;
   if (bias.has_value() && bias->defined()) {
     bias_f = bias->to(torch::kFloat32).contiguous();
@@ -705,7 +636,7 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
     TORCH_CHECK(bias_f.numel() == G * N, "gemm_bf16: bias must be [G, N]");
     p.bias = bias_f.data_ptr<float>();
   }
-  if (aux.has_value() && aux->defined() && aux_mode != 0) {
+  if (has_aux) {
     torch::Tensor ax = aux.value();
     ax = ax.dim() == 2 ? ax.unsqueeze(0) : ax;
     TORCH_CHECK(ax.scalar_type() == torch::kBFloat16 && ax.stride(1) == p.ldc &&
@@ -713,14 +644,6 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
                 "gemm_bf16: aux must be bf16 with the same strides as out");
     TORCH_CHECK(aligned16(ax.data_ptr()), "gemm_bf16: aux must be 16-byte aligned");
     p.aux = reinterpret_cast<const __nv_bfloat16*>(ax.data_ptr());
-  }
-  if (pre_act.has_value() && pre_act->defined()) {
-    torch::Tensor pa = pre_act.value();
-    pa = pa.dim() == 2 ? pa.unsqueeze(0) : pa;
-    TORCH_CHECK(pa.scalar_type() == torch::kBFloat16 && pa.stride(1) == p.ldc &&
-                    (G == 1 || pa.stride(0) == p.c_batch) && aligned16(pa.data_ptr()),
-                "gemm_bf16: pre_act strides");
-    p.pre_act = pa.data_ptr();
   }
   torch::Tensor rs_f;
   if (row_scale.has_value() && row_scale->defined()) {
@@ -731,82 +654,45 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
   if (row_ptrs.has_value() && row_ptrs->defined()) {
     TORCH_CHECK(row_ptrs->scalar_type() == torch::kInt64 && row_ptrs->numel() == G * M &&
                     row_ptrs->is_contiguous(), "gemm_bf16: row_ptrs must be int64 [G, M]");
+    TORCH_CHECK(row_ptrs->is_cuda() && row_ptrs->device() == a_in.device(),
+                "gemm_bf16: row_ptrs must be on the device of a (the kernel reads it)");
     p.row_ptrs = reinterpret_cast<void* const*>(row_ptrs->data_ptr());
   }
-  if (nblk_ptrs.has_value() && nblk_ptrs->defined()) {
-    TORCH_CHECK(nblk_ptrs->scalar_type() == torch::kInt64 && nblk_ptrs->is_cuda() &&
-                    nblk_ptrs->is_contiguous(), "gemm_bf16: nblk_ptrs must be CUDA int64");
-    TORCH_CHECK(G == 1, "gemm_bf16: nblk_ptrs needs G == 1");
-    TORCH_CHECK(!fp32 && N > 128 && nblk_ld > 0 && nblk_ld % 8 == 0 &&
-                    nblk_ptrs->numel() == (N + 255) / 256,
-                "gemm_bf16: nblk_ptrs needs bf16 out, one pointer per 256-column tile and nblk_ld");
-    p.nblk_ptrs = reinterpret_cast<void* const*>(nblk_ptrs->data_ptr());
-    p.ldc = nblk_ld;
-    TORCH_CHECK(p.aux == nullptr && p.pre_act == nullptr, "gemm_bf16: nblk_ptrs excludes aux/pre_act");
-  }
   p.act = static_cast<int>(act);
-  p.aux_mode = p.aux ? static_cast<int>(aux_mode) : 0;
-  p.accumulate = accumulate ? 1 : 0;
-  TORCH_CHECK(!accumulate || fp32, "gemm_bf16: accumulate needs fp32 out");
+  p.aux_mode = has_aux ? static_cast<int>(aux_mode) : kAuxNone;
+  p.epi = p.aux_mode == kAuxAdd ? kEpiAdd
+        : p.aux_mode == kAuxReluMask ? kEpiMask
+        : p.act == kActRelu ? kEpiRelu : kEpiPlain;
 
   if (M == 0 || N == 0 || G == 0) return out;
 
   const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
   const bool bn256 = UseBn256(G, M, N, sms);
   const int bn = bn256 ? 256 : 128;
-  TmapArray ta;
-  if (a_peer_ptrs.has_value() && a_peer_ptrs->defined()) {
-    // `a` is the local K-shard [M, K/W] (K-major); peers hold the other shards at
-    // the given base pointers with identical strides.
-    TORCH_CHECK(a_kmajor && G == 1, "all-gather prologue needs a K-major 2-D A");
-    TORCH_CHECK(a_peer_ptrs->device().is_cpu() && a_peer_ptrs->scalar_type() == torch::kInt64);
-    const int W = static_cast<int>(a_peer_ptrs->numel());
-    TORCH_CHECK(W <= kMaxAMaps);
-    const int64_t k_shard = a.size(2);
-    TORCH_CHECK(k_shard % kBlockK == 0, "K shard must be a multiple of 64");
-    TORCH_CHECK(Kb == k_shard * W, "B's K must equal W * shard K");
-    p.K = static_cast<int>(k_shard * W);
-    p.a_k_per_map = static_cast<int>(k_shard);
-    for (int r = 0; r < W; ++r)
-      ta.m[r] = MakeMap(reinterpret_cast<void*>(a_peer_ptrs->data_ptr<int64_t>()[r]), k_shard, M,
-                        1, a.stride(1), a.stride(1) * a.size(1), kBlockM);
-  } else {
-    ta.m[0] = a_kmajor
-        ? MakeMap(a.data_ptr(), K, M, G, a.stride(1), G > 1 ? a.stride(0) : a.stride(1) * a.size(1), kBlockM)
-        : MakeMap(a.data_ptr(), M, K, G, a.stride(1), G > 1 ? a.stride(0) : a.stride(1) * a.size(1), kBlockK);
-  }
-  CUtensorMap tb = b_kmajor
-      ? MakeMap(b.data_ptr(), Kb, N, G, b.stride(1), G > 1 ? b.stride(0) : b.stride(1) * b.size(1), bn)
-      : MakeMap(b.data_ptr(), N, Kb, G, b.stride(1), G > 1 ? b.stride(0) : b.stride(1) * b.size(1), kBlockK);
+  const CUtensorMap ta = a_kmajor
+      ? MakeMap(a.data_ptr(), K, M, G, a.stride(1), G > 1 ? a.stride(0) : a.stride(1) * a.size(1), kBlockM)
+      : MakeMap(a.data_ptr(), M, K, G, a.stride(1), G > 1 ? a.stride(0) : a.stride(1) * a.size(1), kBlockK);
+  const CUtensorMap tb = b_kmajor
+      ? MakeMap(b.data_ptr(), K, N, G, b.stride(1), G > 1 ? b.stride(0) : b.stride(1) * b.size(1), bn)
+      : MakeMap(b.data_ptr(), N, K, G, b.stride(1), G > 1 ? b.stride(0) : b.stride(1) * b.size(1), kBlockK);
 
-  // Plain bf16 outputs (every site but the redirected-row stores) leave through TMA; the
-  // tensor maps clip ragged M / N edges and follow the row and group strides of C.
-  const bool tma_store = !fp32 && p.row_ptrs == nullptr && p.nblk_ptrs == nullptr &&
-                         p.pre_act == nullptr;
+  // Every output but the redirected-row stores leaves through TMA; the tensor maps clip
+  // ragged M / N edges and follow the row and group strides of C.
+  const bool tma_store = p.row_ptrs == nullptr;
   CUtensorMap tc{}, tx{};
   if (tma_store) {
     const int64_t c_group = G > 1 ? p.c_batch : p.ldc * M;
-    tc = MakeMap(p.c, N, M, G, p.ldc, c_group, 64);
+    tc = MakeMap(out3.data_ptr(), N, M, G, p.ldc, c_group, 64);
     tx = p.aux ? MakeMap(p.aux, N, M, G, p.ldc, c_group, 64) : tc;
-    if (p.aux_mode == kAuxNone)
-      p.epi = p.act == kActNone ? kEpiPlain : p.act == kActRelu ? kEpiRelu : kEpiGeneric;
-    else if (p.act == kActNone && p.aux_mode == kAuxAdd)
-      p.epi = kEpiAdd;
-    else if (p.act == kActNone && p.aux_mode == kAuxReluMask)
-      p.epi = kEpiMask;
-    else
-      p.epi = kEpiGeneric;
   }
 
   cudaStream_t stream = at::cuda::getCurrentCUDAStream();
   if (bn256) {
-    if (fp32) Dispatch<256, float, false>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
-    else if (tma_store) Dispatch<256, __nv_bfloat16, true>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
-    else Dispatch<256, __nv_bfloat16, false>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
+    if (tma_store) Dispatch<256, true>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
+    else Dispatch<256, false>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
   } else {
-    if (fp32) Dispatch<128, float, false>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
-    else if (tma_store) Dispatch<128, __nv_bfloat16, true>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
-    else Dispatch<128, __nv_bfloat16, false>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
+    if (tma_store) Dispatch<128, true>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
+    else Dispatch<128, false>(a_kmajor, b_kmajor, ta, tb, tc, tx, p, sms, stream);
   }
   return out;
 }

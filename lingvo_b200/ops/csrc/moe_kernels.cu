@@ -579,10 +579,6 @@ int64_t symm_import(const std::string& handle, int64_t device) {
   C10_CUDA_CHECK(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
   return reinterpret_cast<int64_t>(p);
 }
-torch::Tensor symm_view(int64_t ptr, int64_t nbytes, int64_t device) {
-  auto opts = torch::TensorOptions().dtype(torch::kUInt8).device(torch::kCUDA, device);
-  return torch::from_blob(reinterpret_cast<void*>(ptr), {nbytes}, opts);
-}
 
 }  // namespace lb
 
@@ -597,5 +593,4 @@ LB_REGISTER(moe) {
   m.def("symm_alloc", &lb::symm_alloc);
   m.def("symm_export", &lb::symm_export);
   m.def("symm_import", &lb::symm_import);
-  m.def("symm_view", &lb::symm_view);
 }

@@ -18,8 +18,8 @@ import torch.nn.functional as F
 
 from lingvo_b200 import ops
 
-ACT_IDS = {None: 0, 'NONE': 0, 'RELU': 1, 'GELU': 2, 'SILU': 3, 'SWISH': 3,
-           'GELU_APPROXIMATE': 4, 'SQUARED_RELU': 5}
+# The GEMM epilogue fuses ReLU only; callers apply other activations after it.
+ACT_IDS = {None: 0, 'NONE': 0, 'RELU': 1}
 AUX_NONE, AUX_RELU_MASK, AUX_ADD = 0, 1, 2
 
 
@@ -29,14 +29,6 @@ def _act_ref(x, act):
     return x
   if a == 1:
     return F.relu(x)
-  if a == 2:
-    return F.gelu(x)
-  if a == 3:
-    return F.silu(x)
-  if a == 4:
-    return F.gelu(x, approximate='tanh')
-  if a == 5:
-    return F.relu(x).square()
   raise ValueError(act)
 
 
@@ -63,24 +55,20 @@ def gemm_ref(a, b, a_kmajor=True, b_kmajor=True, bias=None, act=0, aux=None,
 
 
 def gemm(a, b, a_kmajor=True, b_kmajor=True, bias=None, act=0, aux=None,
-         aux_mode=0, row_scale=None, out=None, out_fp32=False,
-         accumulate=False, pre_act=None, row_ptrs=None, nblk_ptrs=None,
-         a_peer_ptrs=None, nblk_ld=0):
-  """C[g] = epi(A[g] · B[g]^T); see csrc/gemm_wgmma.cu for operand layouts."""
+         aux_mode=0, row_scale=None, out=None, row_ptrs=None):
+  """bf16 C[g] = epi(A[g] · B[g]^T); see csrc/gemm_wgmma.cu for operand layouts.
+
+  `row_ptrs` (int64 [G·M] on the device) redirects each output row to the
+  given address (0 skips the row)."""
   act = ACT_IDS[act] if not isinstance(act, int) else act
   if not ops.use_cuda_kernels(a, b):
-    y = gemm_ref(a, b, a_kmajor, b_kmajor, bias, act, aux, aux_mode, row_scale,
-                 out_fp32 or (out is not None and out.dtype == torch.float32))
+    y = gemm_ref(a, b, a_kmajor, b_kmajor, bias, act, aux, aux_mode, row_scale)
     if out is not None:
-      if accumulate:
-        out.add_(y.reshape(out.shape))
-      else:
-        out.copy_(y.reshape(out.shape))
+      out.copy_(y.reshape(out.shape))
       return out
     return y
   res = ops.native().gemm_bf16(a, b, a_kmajor, b_kmajor, bias, act, aux,
-                               aux_mode, row_scale, out, out_fp32, accumulate,
-                               pre_act, row_ptrs, nblk_ptrs, a_peer_ptrs, nblk_ld)
+                               aux_mode, row_scale, out, row_ptrs)
   if out is None and a.dim() == 2:
     res = res[0]
   return res
@@ -100,9 +88,6 @@ class _LinearFn(torch.autograd.Function):
     ctx.has_res = residual is not None
     ctx.act_id = act_id
     ctx.has_bias = bias is not None
-    if act_id not in (0, 1):
-      raise NotImplementedError('fused backward supports NONE/RELU; use '
-                                'linear(..., act=None) + activation for others')
     ctx.save_for_backward(x, w, y if act_id == 1 else None)
     return y
 
@@ -117,8 +102,7 @@ class _LinearFn(torch.autograd.Function):
     if ctx.needs_input_grad[0]:
       dx = gemm(dy, w, True, True)                      # dy @ w^T
     if ctx.needs_input_grad[1]:
-      dw = gemm(x, dy, False, False, out_fp32=(w.dtype == torch.float32))
-      dw = dw.to(w.dtype)
+      dw = gemm(x, dy, False, False)
     if ctx.has_bias and ctx.needs_input_grad[2]:
       db = dy.float().sum(dim=-2)
     return dx, dw, db, None, (dy if ctx.has_res else None)

@@ -14,10 +14,7 @@ column-parallel GEMM (weights split on the output dim) followed by a row-paralle
     identity backward.
 
 Both run on `ctx.tp_group` (NCCL over NVLink on the device, gloo in CPU tests). The local
-GEMMs are the framework's wgmma kernels. The fully fused variant — collectives inside the
-GEMM kernel over peer memory — lives in `parallel/tp.py` (`TpEngine`); it is selected with
-`LINGVO_B200_TP_FUSED=1` for geometries it supports and is otherwise an experimental path:
-the NCCL + wgmma-GEMM composition is the default.
+GEMMs are the framework's wgmma kernels.
 """
 
 from __future__ import annotations

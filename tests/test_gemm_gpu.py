@@ -2,6 +2,7 @@
 import pytest
 import torch
 
+from lingvo_b200 import ops
 from lingvo_b200.ops import gemm as G
 
 pytestmark = pytest.mark.gpu
@@ -30,7 +31,7 @@ def test_layouts(ak, bk, m, n, k):
   _check(y, G.gemm_ref(a, b, ak, bk, out_fp32=True), k)
 
 
-def test_grouped_and_epilogue():
+def test_grouped_and_bf16_epilogues():
   g, m, n, k = 8, 320, 512, 256
   a = _mk((g, m, k), seed=3)
   b = _mk((g, k, n), seed=4)
@@ -41,12 +42,39 @@ def test_grouped_and_epilogue():
   y = G.gemm(a, b, True, False, aux=aux, aux_mode=G.AUX_RELU_MASK)
   _check(y, G.gemm_ref(a, b, True, False, aux=aux, aux_mode=1, out_fp32=True), k)
   rs = torch.rand(g, m, device='cuda')
-  y = G.gemm(a, b, True, False, row_scale=rs, out_fp32=True)
-  assert y.dtype == torch.float32
+  y = G.gemm(a, b, True, False, row_scale=rs)
+  assert y.dtype == torch.bfloat16
   _check(y, G.gemm_ref(a, b, True, False, row_scale=rs, out_fp32=True), k)
-  acc = torch.ones(g, m, n, device='cuda')
-  G.gemm(a, b, True, False, out=acc, accumulate=True)
-  _check(acc, G.gemm_ref(a, b, True, False, out_fp32=True) + 1.0, k)
+
+
+def test_unsupported_epilogues_are_rejected_without_launching():
+  """Only NONE / RELU are fused, ReLU takes no aux operand, and the kernel reads the
+  row-pointer table, so a host table is refused. The oracle refuses the same activations."""
+  m, n, k = 256, 256, 128
+  a = _mk((m, k), seed=9)
+  b = _mk((k, n), seed=10)
+  aux = _mk((m, n), seed=11)
+  out = torch.empty(m, n, device='cuda', dtype=torch.bfloat16)
+  host_ptrs = out.data_ptr() + torch.arange(m, dtype=torch.int64) * (n * 2)
+  nat = ops.native()
+  launches = nat.launch_count()
+  with pytest.raises(KeyError):
+    G.gemm(a, b, True, False, act='GELU')
+  with pytest.raises(RuntimeError, match='act'):
+    G.gemm(a, b, True, False, act=2)
+  for mode in (G.AUX_ADD, G.AUX_RELU_MASK):
+    with pytest.raises(RuntimeError, match='ReLU'):
+      G.gemm(a, b, True, False, act=1, aux=aux, aux_mode=mode)
+  with pytest.raises(RuntimeError, match='row_ptrs'):
+    G.gemm(a, b, True, False, out=out, row_ptrs=host_ptrs)
+  assert nat.launch_count() == launches
+  ac, bc = a.cpu(), b.cpu()
+  with pytest.raises(KeyError):
+    G.gemm(ac, bc, True, False, act='GELU')
+  with pytest.raises(KeyError):
+    G.gemm_ref(ac, bc, True, False, act='GELU')
+  with pytest.raises(ValueError):
+    G.gemm_ref(ac, bc, True, False, act=2)
 
 
 def test_linear_autograd():

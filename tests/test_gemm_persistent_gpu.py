@@ -39,16 +39,17 @@ def test_layouts_and_schedules(g, m, n, k, ak, bk):
   _close(G.gemm(a, b, ak, bk), G.gemm_ref(a, b, ak, bk, out_fp32=True))
 
 
-@pytest.mark.parametrize('act', [1, 2, 3, 4, 5])
-def test_bias_and_activations(act):
+@pytest.mark.parametrize('ak,bk', [(True, True), (True, False), (False, True), (False, False)])
+@pytest.mark.parametrize('act', [0, 1])
+def test_bias_and_activations(act, ak, bk):
   g, m, n, k = _G, _M, _N, _K
-  a, b = _operands(g, m, n, k, True, False, seed=3)
+  a, b = _operands(g, m, n, k, ak, bk, seed=3)
   bias = torch.randn(g, n, device='cuda')
-  y = G.gemm(a, b, True, False, bias=bias, act=act)
-  _close(y, G.gemm_ref(a, b, True, False, bias=bias, act=act, out_fp32=True))
+  y = G.gemm(a, b, ak, bk, bias=bias, act=act)
+  _close(y, G.gemm_ref(a, b, ak, bk, bias=bias, act=act, out_fp32=True))
 
 
-def test_aux_row_scale_pre_act_accumulate():
+def test_aux_and_row_scale():
   g, m, n, k = _G, _M, _N, _K
   a, b = _operands(g, m, n, k, True, True, seed=5)
   aux = _mk((g, m, n), seed=7)
@@ -57,17 +58,8 @@ def test_aux_row_scale_pre_act_accumulate():
     _close(y, G.gemm_ref(a, b, True, True, aux=aux, aux_mode=mode, out_fp32=True))
   rs = torch.rand(g, m, device='cuda')
   a2, b2 = _operands(g, m, n, k, False, False, seed=9)
-  y = G.gemm(a2, b2, False, False, row_scale=rs, out_fp32=True)
+  y = G.gemm(a2, b2, False, False, row_scale=rs)
   _close(y, G.gemm_ref(a2, b2, False, False, row_scale=rs, out_fp32=True))
-  bias = torch.randn(g, n, device='cuda')
-  pre = torch.empty(g, m, n, device='cuda', dtype=torch.bfloat16)
-  y = G.gemm(a, b, True, True, bias=bias, act=1, pre_act=pre)
-  _close(pre, G.gemm_ref(a, b, True, True, bias=bias, out_fp32=True))
-  _close(y, G.gemm_ref(a, b, True, True, bias=bias, act=1, out_fp32=True))
-  acc = torch.randn(g, m, n, device='cuda')
-  ref = G.gemm_ref(a, b, True, True, out_fp32=True) + acc
-  G.gemm(a, b, True, True, out=acc, accumulate=True)
-  _close(acc, ref)
 
 
 def test_row_ptrs_with_null_rows():

@@ -1,9 +1,9 @@
-"""TMA-store epilogue of the wgmma GEMM: bitwise equal to the general epilogue.
+"""TMA-store epilogue of the wgmma GEMM: bitwise equal to the general (row-pointer) epilogue.
 
-A plain bf16 output leaves through TMA bulk stores; asking for a pre-activation tap (or
-redirected rows) routes the same GEMM through the general st.global epilogue, whose
-per-element arithmetic is the same. So the two must agree bit for bit, for every fused
-epilogue, ragged edge, group layout and output stride.
+A plain bf16 output leaves through TMA bulk stores; redirected rows route the same GEMM
+through the general st.global epilogue, whose per-element arithmetic is the same. So the
+two must agree bit for bit, for every fused epilogue, ragged edge, group layout and output
+stride.
 """
 import pytest
 import torch
@@ -25,11 +25,13 @@ def _operands(g, m, n, k, ak, bk, seed=0):
 
 
 def _general(a, b, ak, bk, **kw):
-  """Same GEMM through the general epilogue (the pre-activation tap forces it)."""
+  """Same GEMM through the general epilogue, forced by an identity row-pointer table."""
   g, m = (a.shape[0], a.shape[1] if ak else a.shape[2])
   n = b.shape[1] if bk else b.shape[2]
-  tap = torch.empty(g, m, n, device='cuda', dtype=torch.bfloat16)
-  return G.gemm(a, b, ak, bk, pre_act=tap, **kw)
+  out = torch.empty(g, m, n, device='cuda', dtype=torch.bfloat16)
+  rows = torch.arange(g * m, device='cuda', dtype=torch.int64)
+  G.gemm(a, b, ak, bk, row_ptrs=out.data_ptr() + rows * (n * 2), **kw)
+  return out
 
 
 # (G, M, N, K) on a 132-SM H100: an odd number of M-tiles with ragged M and N (776 =
@@ -43,12 +45,12 @@ _SHAPES = [(1, 776, 840, 256), (3, 200, 640, 256), (1, 1024, 2048, 2048), (1, 20
 _EPILOGUES = {
     'plain': {},
     'relu': dict(act=1),
-    'gelu': dict(act=2),
     'bias_relu': dict(act=1, bias=True),
     'residual': dict(aux_mode=G.AUX_ADD),
     'relu_mask': dict(aux_mode=G.AUX_RELU_MASK),
     'row_scale': dict(row_scale=True),
     'bias_residual_row_scale': dict(aux_mode=G.AUX_ADD, bias=True, row_scale=True),
+    'bias_relu_mask_row_scale': dict(aux_mode=G.AUX_RELU_MASK, bias=True, row_scale=True),
 }
 
 
@@ -65,7 +67,7 @@ def _kwargs(spec, g, m, n, seed):
 
 @pytest.mark.parametrize('epi', list(_EPILOGUES))
 @pytest.mark.parametrize('g,m,n,k', _SHAPES)
-def test_tma_store_matches_general_epilogue(g, m, n, k, epi):
+def test_tma_store_matches_row_pointer_epilogue(g, m, n, k, epi):
   ak, bk = (True, True) if epi in ('relu_mask', 'plain') else (True, False)
   a, b = _operands(g, m, n, k, ak, bk, seed=21)
   kw = _kwargs(_EPILOGUES[epi], g, m, n, seed=23)
@@ -76,7 +78,7 @@ def test_tma_store_matches_general_epilogue(g, m, n, k, epi):
   assert err / (ref.abs().max().item() + 1e-6) < 2e-2
 
 
-def test_wgrad_majors_match_general_epilogue():
+def test_wgrad_majors_match_row_pointer_epilogue():
   a, b = _operands(4, 904, 1024, 512, False, False, seed=31)
   rs = torch.rand(4, 904, device='cuda')
   y = G.gemm(a, b, False, False, row_scale=rs)

@@ -32,13 +32,6 @@ def test_fused_ep_dp_matches_nccl_baseline():
   assert rc == 0 and 'MGPU_OK' in out, out[-3000:]
 
 
-def test_tensor_parallel_ffn_matches_oracle():
-  """TP FFN with collectives fused into the wgmma GEMM vs fp32 single-device oracle."""
-  _NeedGpus(2)
-  rc, out = _Run('tools/tp_check.py', 2, 29622, '2048', '1024', '2048')
-  assert rc == 0 and 'TP_OK' in out, out[-3000:]
-
-
 def test_product_trainer_two_gpus_identical_replicas_resume_and_gradients():
   """`runners.Trainer` under torchrun: replicated weights identical across ranks after 10
   steps, sharded checkpoint + resume, and per-variable gradients fused ≈ NCCL baseline."""
