@@ -454,13 +454,15 @@ class SelfAttentionLayer(_BuilderLayer):
       return (out + residual if residual is not None else out), aux
     return self._FPropLocal(theta, x, segment_id, segment_pos, residual)
 
-  def _FPropLocal(self, theta, x, segment_id, segment_pos, residual=None):
+  def _ProjectQkv(self, theta, x, segment_id, segment_pos):
+    """x `[B,L,M]` → q `[B,L,H,D]`, k / v `[B,L,Hk,D]` of this rank's heads, after the
+    multi-dconv-head convolutions and RoPE."""
     b = self.bp
-    bsz, l, m = x.shape
+    bsz, l, _ = x.shape
     d = b.attention_key_value_dim
     h, hk = self._LocalHeads()
     from lingvo_b200.ops import gemm
-    wq, wk, wv, wo = theta.wq, theta.wk, theta.wv, theta.wo
+    wq, wk, wv = theta.wq, theta.wk, theta.wv
     if b.attention_combine_qkv and hk == h:
       wqkv = torch.cat([wq, wk, wv], dim=1)
       qkv = gemm.linear(x, wqkv.to(x.dtype))
@@ -480,6 +482,16 @@ class SelfAttentionLayer(_BuilderLayer):
     if b.use_rotary_position_emb or (self.params.multi_dconv_head and b.mdha_rope):
       q = _Rope(q, segment_pos, b.rope_emb_max_timescale)
       k = _Rope(k, segment_pos, b.rope_emb_max_timescale)
+    return q, k, v
+
+  def _FPropLocal(self, theta, x, segment_id, segment_pos, residual=None):
+    b = self.bp
+    bsz, l, _ = x.shape
+    d = b.attention_key_value_dim
+    h, _ = self._LocalHeads()
+    from lingvo_b200.ops import gemm
+    wo = theta.wo
+    q, k, v = self._ProjectQkv(theta, x, segment_id, segment_pos)
     if _ContextParallel(b):
       o = self._ContextParallelCore(theta, q, k, v, segment_id)
       out = gemm.linear(o.reshape(bsz, l, h * d), wo.to(x.dtype), residual=residual)
@@ -547,13 +559,7 @@ def _SelfAttentionExtendStep(layer, theta, x, cache, t):
   else:
     # Fused cache append + attention over the live keys (our split-KV kernel on the GPU).
     from lingvo_b200.ops import attention as attention_ops
-    rel = None
-    if layer.params.relative_bias:
-      bucket = RelativePositionBucket(     # table[:, i] for key − query = T − 1 − i
-          torch.arange(tmax - 1, -tmax, -1, device=dev), b.relative_attention_num_buckets,
-          b.relative_attention_max_distance,
-          bidirectional=b.decoder_bidirectional_relative_attention)
-      rel = theta.wrb.float()[:, bucket.long()]
+    rel = _DecodeRelTable(layer, theta, tmax, dev)
     o = attention_ops.decode_attention(q, k, v, cache.k, cache.v, tt, rel)
     o = o.reshape(bsz, 1, h * d)
   out = torch.matmul(o, theta.wo.to(xd))
@@ -561,6 +567,82 @@ def _SelfAttentionExtendStep(layer, theta, x, cache, t):
     from lingvo_b200.parallel import tp_layers   # pylint: disable=g-import-not-at-top
     out = tp_layers.ReduceFromTensorParallel(out, layer._tp)   # pylint: disable=protected-access
   return out
+
+
+def _DecodeRelTable(layer, theta, tmax, dev):
+  """fp32 `[H, 2T-1]` relative-bias table of a decode step over a `T`-row cache, indexed by
+  query − key + T − 1; None for a layer without relative bias."""
+  if not layer.params.relative_bias:
+    return None
+  b = layer.bp
+  bucket = RelativePositionBucket(     # table[:, i] for key − query = T − 1 − i
+      torch.arange(tmax - 1, -tmax, -1, device=dev), b.relative_attention_num_buckets,
+      b.relative_attention_max_distance,
+      bidirectional=b.decoder_bidirectional_relative_attention)
+  return theta.wrb.float()[:, bucket.long()]
+
+
+def _SelfAttentionOut(layer, theta, o, xd):
+  """Output projection of the attended heads `[B, L, H·D]` of a decode call."""
+  out = torch.matmul(o, theta.wo.to(xd))
+  if layer._tp is not None:   # pylint: disable=protected-access
+    from lingvo_b200.parallel import tp_layers   # pylint: disable=g-import-not-at-top
+    out = tp_layers.ReduceFromTensorParallel(out, layer._tp)   # pylint: disable=protected-access
+  return out
+
+
+def _SelfAttentionPrefill(layer, theta, x, segment_id, segment_pos, cache):
+  """The whole prompt x `[B,P,M]` in one call: writes the post-RoPE keys / values into cache
+  rows [0, P) and the positions into `cache.pos`, and returns the block output `[B,P,M]`.
+  Pads carry segment id 0: they see nothing and nothing sees them. Where the layer's forward
+  takes our flash kernel, so does this call (P padded to a multiple of 128); elsewhere it
+  takes the layer's fp32 path."""
+  b = layer.bp
+  bsz, plen, _ = x.shape
+  d = b.attention_key_value_dim
+  h, _ = layer._LocalHeads()   # pylint: disable=protected-access
+  q, k, v = layer._ProjectQkv(theta, x, segment_id, segment_pos)   # pylint: disable=protected-access
+  cache.k[:, :plen] = k.to(cache.k.dtype)
+  cache.v[:, :plen] = v.to(cache.v.dtype)
+  cache.pos[:, :plen] = segment_pos.to(cache.pos.dtype)
+  from lingvo_b200.ops import attention as attention_ops
+  simple = (not b.atten_logit_cap) and b.attention_extra_logit is None
+  toeplitz = (not layer.params.relative_bias) or b.relative_attention_use_universal_1d_position
+  causal = layer.params.decoder and not b.decoder_skip_causal_mask
+  pad = -plen % 128
+  padded = [F.pad(t, (0, 0, 0, 0, 0, pad)) for t in (q, k, v)]
+  if simple and toeplitz and attention_ops.flash_attention_supported(padded[0], padded[1]):
+    rel = layer._RelTable(theta, plen + pad, x.device) if layer.params.relative_bias else None   # pylint: disable=protected-access
+    o = attention_ops.flash_attention(*padded, rel, F.pad(segment_id, (0, pad)),
+                                      F.pad(segment_pos, (0, pad)), 1.0, causal)[:, :plen]
+  else:
+    bias = layer._Bias(theta, segment_id, segment_pos, torch.float32)   # pylint: disable=protected-access
+    o = _AttentionCore(q, k, v, bias, b.atten_logit_cap, b.attention_extra_logit)
+  return _SelfAttentionOut(layer, theta, o.reshape(bsz, plen, h * d), x.dtype)
+
+
+def _SelfAttentionBeamStep(layer, theta, x, cache, slot0, vis, qpos):
+  """One flat-beam-search step: x `[B,K,M]` holds one token per hypothesis at positions
+  `qpos [B,K]`. Appends their keys / values at cache rows slot0 … slot0+K-1 and lets
+  hypothesis k attend over the rows set in its bit mask `vis [B,K,⌈N/32⌉]`."""
+  b = layer.bp
+  bsz, kk, _ = x.shape
+  d = b.attention_key_value_dim
+  h, hk = layer._LocalHeads()   # pylint: disable=protected-access
+  xd = x.dtype
+  q = torch.matmul(x, theta.wq.to(xd)).reshape(bsz, kk, h, d)
+  k = torch.matmul(x, theta.wk.to(xd)).reshape(bsz, kk, hk, d)
+  v = torch.matmul(x, theta.wv.to(xd)).reshape(bsz, kk, hk, d)
+  if b.use_rotary_position_emb:
+    q, k = _Rope(q, qpos, b.rope_emb_max_timescale), _Rope(k, qpos, b.rope_emb_max_timescale)
+  tmax = cache.k.shape[1]
+  rows = torch.as_tensor(slot0, device=x.device).reshape(()) + torch.arange(kk, device=x.device)
+  cache.pos.scatter_(1, rows.unsqueeze(0).expand(bsz, kk), qpos.to(cache.pos.dtype))
+  from lingvo_b200.ops import attention as attention_ops
+  o = attention_ops.flat_beam_attention(
+      q, k, v, cache.k, cache.v, slot0, vis, qpos, cache.pos,
+      _DecodeRelTable(layer, theta, tmax, x.device), 1.0, b.atten_logit_cap)
+  return _SelfAttentionOut(layer, theta, o.reshape(bsz, kk, h * d), xd)
 
 
 def _CappedDecodeAttention(layer, theta, q, k, v, cache, tt):
@@ -1133,6 +1215,76 @@ class LayerStack(_BuilderLayer):
       if getattr(blk.layer, 'needs_encoder', False):
         kvs[idx] = blk.layer.ProjectEncoder(theta.layers[idx].layer, encoder_output)
     return NestedMap(kv=kvs, segment_id=encoder_segment_id)
+
+  def _CheckBeamSupported(self):
+    """Prefill / BeamExtendStep handle self-attention (without multi-dconv heads) and
+    position-wise blocks only; anything else would decode wrongly, so it is refused."""
+    for blk in self.layers:
+      lyr = blk.layer
+      if isinstance(lyr, SelfAttentionLayer):
+        if lyr.params.multi_dconv_head:
+          raise NotImplementedError(
+              '%s: multi-dconv-head attention cannot be prefilled or beam-stepped' %
+              blk.params.name)
+      elif not isinstance(lyr, (DenseReluDenseLayer, MoELayer)):
+        raise NotImplementedError(
+            '%s: %s cannot be prefilled or beam-stepped; only self-attention and '
+            'feed-forward / MoE blocks can' % (blk.params.name, type(lyr).__name__))
+
+  def _RunBlocks(self, theta, x, attend, seg, pos):
+    """The ExtendStep block loop over x `[R, L, M]`: self-attention blocks call
+    `attend(layer, theta, y, cache)`, the others run on `seg` / `pos` `[R, L]`."""
+    for idx, blk in enumerate(self.layers):
+      th = theta.layers[idx]
+      y = blk.ln.FProp(th.ln, x)
+      if isinstance(blk.layer, SelfAttentionLayer):
+        y = attend(blk.layer, th.layer, y, idx)
+      else:
+        y, _ = blk.layer.FProp(th.layer, y, seg, pos)
+      if blk.params.residual_weight != 1.0:
+        y = y * blk.params.residual_weight
+      if blk.params.post_norm is not None:
+        y = blk.post_ln.FProp(th.post_ln, y)
+      x = x + y
+    if 'final_layer_norm' in self.children:
+      x = self.final_layer_norm.FProp(theta.final_layer_norm, x)
+    return x
+
+  def Prefill(self, theta, vec, segment_id, segment_pos, state):
+    """Runs a prompt `vec [B,P,M]` through the stack in one call and writes every
+    self-attention block's keys / values into cache rows [0, P) of `state` (from
+    `InitDecodeState`). Tokens with `segment_id` 0 are padding. Returns `[B,P,M]`."""
+    self._CheckBeamSupported()
+    bsz, plen, _ = vec.shape
+    for cache in state:
+      if cache is not None:
+        assert plen <= cache.k.shape[1], (plen, cache.k.shape)
+        cache.pos = torch.zeros(bsz, cache.k.shape[1], dtype=torch.int32, device=vec.device)
+
+    def Attend(layer, th, y, idx):
+      return _SelfAttentionPrefill(layer, th, y, segment_id, segment_pos, state[idx])
+    return self._RunBlocks(theta, vec, Attend, segment_id, segment_pos)
+
+  def BeamExtendStep(self, theta, vec, state, slot0, vis, qpos):
+    """One flat-beam-search step after `Prefill`: `vec [B,K,M]` holds the token of each of
+    the K hypotheses at positions `qpos [B,K]`; they are appended at cache rows
+    slot0 … slot0+K-1 (slot0 a Python int or 0-dim device tensor), and hypothesis k attends
+    over the rows set in its int32 bit mask `vis [B,K,⌈N/32⌉]` (`ops.attention.
+    pack_visibility`). Every other block sees B·K rows of one token, as in `ExtendStep`, so
+    no hypothesis depends on its siblings. Returns `[B,K,M]`."""
+    self._CheckBeamSupported()
+    bsz, kk, m = vec.shape
+    for cache in state:
+      if cache is not None and 'pos' not in cache:
+        raise ValueError('BeamExtendStep needs a state filled by Prefill')
+    seg = torch.ones(bsz * kk, 1, dtype=torch.long, device=vec.device)
+    pos = qpos.reshape(bsz * kk, 1).long()
+
+    def Attend(layer, th, y, idx):
+      return _SelfAttentionBeamStep(layer, th, y.reshape(bsz, kk, m), state[idx], slot0, vis,
+                                    qpos).reshape(bsz * kk, 1, m)
+    return self._RunBlocks(theta, vec.reshape(bsz * kk, 1, m), Attend, seg, pos).reshape(
+        bsz, kk, m)
 
   def ExtendStep(self, theta, vec, state, t, encoder_state=None):
     """vec `[B,1,M]` at position t → `[B,1,M]`; `state` from `InitDecodeState`."""
@@ -1902,26 +2054,55 @@ class UniTransformer(base_model.BaseTask):
   def InitDecodeState(self, batch, max_len, device):
     return self.dec.InitDecodeState(batch, max_len, device, self.fprop_dtype)
 
-  def DecodeStep(self, theta, ids, state, t):
-    """ids `[B]` at position t → logits `[B, V]` (fp32); updates `state` in place."""
+  def _EmbedDecodeIds(self, theta, ids, pos):
+    """Token + positional embedding of ids `[B, L]` at positions `[B, L]`."""
     p = self.params
     fd = self.fprop_dtype
-    y = self.dec_emb.FProp(theta.dec_emb, ids.reshape(-1, 1)).to(fd)
+    y = self.dec_emb.FProp(theta.dec_emb, ids).to(fd)
     if p.positional_embedding:
-      pos = torch.as_tensor(t, device=y.device).reshape(1, 1).expand(y.shape[0], 1)
       if p.sinusoid_positional_embedding:
         y = y + self.dec_pos_emb.FPropWithPosition(theta.dec_pos_emb, pos).to(fd)
       else:
         y = y + self.dec_pos_emb.FProp(theta.dec_pos_emb, pos).to(fd)
-    out = self.dec.ExtendStep(theta.dec, y, state, t)
+    return y
+
+  def _DecodeLogits(self, theta, out):
+    p = self.params
     if p.scale_decoder_outputs:
       out = out * (p.builder.model_dim ** -0.5)
-    return self._ComputeLogits(theta, out).float().squeeze(1)
+    return self._ComputeLogits(theta, out).float()
+
+  def DecodeStep(self, theta, ids, state, t):
+    """ids `[B]` at position t → logits `[B, V]` (fp32); updates `state` in place."""
+    ids = ids.reshape(-1, 1)
+    pos = torch.as_tensor(t, device=ids.device).reshape(1, 1).expand(ids.shape[0], 1)
+    y = self._EmbedDecodeIds(theta, ids, pos)
+    out = self.dec.ExtendStep(theta.dec, y, state, t)
+    return self._DecodeLogits(theta, out).squeeze(1)
+
+  def Prefill(self, theta, ids, segment_id, segment_pos, state):
+    """Writes a prompt `ids [B, P]` (padding: segment id 0) into the caches of `state` (from
+    `InitDecodeState`) in one pass through the stack. No LM head runs on the prompt."""
+    y = self._EmbedDecodeIds(theta, ids, segment_pos)
+    self.dec.Prefill(theta.dec, y, segment_id, segment_pos, state)
+
+  def BeamDecodeStep(self, theta, ids, pos, state, slot0, vis):
+    """One flat-beam-search step after `Prefill`: ids `[B, K]` at positions `pos [B, K]`,
+    appended at cache rows slot0 … slot0+K-1; hypothesis k sees the rows of its bit mask
+    `vis [B, K, ⌈N/32⌉]`. Returns logits `[B, K, V]` (fp32)."""
+    y = self._EmbedDecodeIds(theta, ids, pos)
+    out = self.dec.BeamExtendStep(theta.dec, y, state, slot0, vis, pos)
+    return self._DecodeLogits(theta, out)
 
   def Decode(self, input_batch):
-    """Greedy / beam decode of continuations (see gshard_decode)."""
+    """Greedy / sampled decode of continuations (see gshard_decode)."""
     from lingvo_b200.core import gshard_decode
     return gshard_decode.DecodeIds(self, self.theta, input_batch)
+
+  def BeamDecode(self, input_batch):
+    """Flat beam search of continuations with `decoder_beam_size` hypotheses."""
+    from lingvo_b200.core import gshard_decode
+    return gshard_decode.BeamDecodeIds(self, self.theta, input_batch)
 
 
 class TunableUniTransformer(UniTransformer):

@@ -177,6 +177,14 @@ class GShardDecode:
     self._stop.set()
 
 
+def _PrefixLens(tgt):
+  if 'paddings' in tgt:
+    plen = (1.0 - tgt.paddings.float()).sum(1).long()
+  else:
+    plen = (tgt.segment_ids != 0).sum(1).long()
+  return plen.clamp_min(1)
+
+
 def DecodeIds(task, theta, input_batch, max_steps=None, temperature=0.0, top_k=0, seed=0):
   """Continues every row of a prefix batch with the task's incremental decoder (greedy,
   or temperature / top-k sampling) (ref :186 `_DecodeStep` + `gshard_builder` decode).
@@ -191,11 +199,7 @@ def DecodeIds(task, theta, input_batch, max_steps=None, temperature=0.0, top_k=0
   ids = tgt.ids.long()
   b, t0 = ids.shape
   dev = ids.device
-  if 'paddings' in tgt:
-    plen = (1.0 - tgt.paddings.float()).sum(1).long()
-  else:
-    plen = (tgt.segment_ids != 0).sum(1).long()
-  plen = plen.clamp_min(1)
+  plen = _PrefixLens(tgt)
   steps = int(max_steps or p.decoder_max_steps)
   total = t0 + steps
   out = torch.full((b, total), int(p.decoder_eos_id), dtype=torch.long, device=dev)
@@ -231,3 +235,44 @@ def DecodeIds(task, theta, input_batch, max_steps=None, temperature=0.0, top_k=0
       if (t + 1) % 8 == 0 and t + 1 >= int(t0) and bool(done.all()):
         break
   return NestedMap(ids=out, prefix_lens=plen, lens=lens, scores=scores)
+
+
+def BeamDecodeIds(task, theta, input_batch, beam_size=None, max_steps=None):
+  """Flat beam search from every row's prefix (ref `gshard_builder.DecodeIds` with
+  `_FlatBeamSearchCallback`): the prompts are right-aligned and written into the KV caches
+  in one `task.Prefill` call, then each `task.BeamDecodeStep` extends all K hypotheses of a
+  row in the shared token buffer, each attending over its own prompt and ancestors.
+
+  `input_batch.tgt.ids [B, T]` with `paddings` (or `segment_ids`) marking each prefix, as for
+  `DecodeIds`. `beam_size` / `max_steps` default to `decoder_beam_size` / `decoder_max_steps`.
+  Returns NestedMap(topk_ids [B, K, S] (continuations only, EOS-terminated), topk_lens
+  [B, K] (0 for an empty slot), topk_scores [B, K] (length-normalised log-probabilities,
+  best first), prefix_lens [B])."""
+  from lingvo_b200.core import flat_beam_search_helper as fbs
+  from lingvo_b200.core.nested_map import NestedMap
+  from lingvo_b200.ops import attention as attention_ops
+  p = task.params
+  tgt = input_batch.tgt if 'tgt' in input_batch else input_batch
+  ids = tgt.ids.long()
+  b, t0 = ids.shape
+  dev = ids.device
+  plen = _PrefixLens(tgt)
+  k = int(beam_size or p.decoder_beam_size)
+  steps = int(max_steps or p.decoder_max_steps)
+  pmax = -(-t0 // k) * k
+  src = torch.arange(pmax, device=dev) - (pmax - plen).unsqueeze(1)   # right-aligned prompts
+  prefix = torch.where(src >= 0, ids.gather(1, src.clamp(0, t0 - 1)), torch.zeros_like(src))
+
+  def Callback(tgt_id, tgt_pos, tgt_segment_id, tgt_mask, state, t):
+    if tgt_mask is None:
+      task.Prefill(theta, tgt_id, tgt_segment_id, tgt_pos, state)
+      return None, state
+    vis = attention_ops.pack_visibility(tgt_mask)
+    return task.BeamDecodeStep(theta, tgt_id, tgt_pos, state, t * k, vis), state
+
+  with torch.no_grad():
+    state = task.InitDecodeState(b, pmax + k * steps, dev)
+    (out, lens, scores), _ = fbs.flat_beam_search(
+        b, k, steps, Callback, state, eos_id=int(p.decoder_eos_id), prefix=prefix,
+        prefix_len=plen, device=dev)
+  return NestedMap(topk_ids=out, topk_lens=lens, topk_scores=scores, prefix_lens=plen)

@@ -2,13 +2,16 @@
 
   python -m lingvo_b200.models.lm.tools.gshard_lm_decode \
       --model=lm.synthetic_packed_input.DenseLm8B2x2Decode --checkpoint=/path/ckpt-00001000 \
-      --input=prompts.tsv --output=continuations.tsv --batch_size=16 --prefix_max_len=128
+      --input=prompts.tsv --output=continuations.tsv --batch_size=16 --prefix_max_len=128 \
+      [--beam_size=4]
 
 `GShardLMDecode` serves prompts through the stream-pipelined loop of
 `core.gshard_decode.GShardDecode` (pinned H2D infeed → device decode → D2H outfeed);
 `GShardLMDecodeBatch` decodes whole TSV files (one prompt per line, space-separated token
 ids unless a tokenizer is plugged in by overriding `init_vocab / encode_string_to_ids /
-decode_ids_to_string`) and skips files already decoded (restart-safe).
+decode_ids_to_string`) and skips files already decoded (restart-safe). With `beam_size` ≥ 1
+the continuations come from a flat beam search (`gshard_decode.BeamDecodeIds`) and each line
+holds the best hypothesis and its length-normalised score; 0 keeps greedy / sampled decoding.
 """
 
 from __future__ import annotations
@@ -52,8 +55,10 @@ class GShardLMDecode(gshard_decode.GShardDecode):
   """Interactive / streaming decoder (ref :82)."""
 
   def __init__(self, model_name, checkpoint=None, prefix_max_len=128, batch_size=8,
-               max_decode_steps=None, temperature=0.0, device=None, params_override=''):
+               max_decode_steps=None, temperature=0.0, device=None, params_override='',
+               beam_size=0):
     self.prefix_max_len = prefix_max_len
+    self.beam_size = beam_size
     self.batch_size = batch_size
     self.temperature = temperature
     try:
@@ -114,6 +119,12 @@ class GShardLMDecode(gshard_decode.GShardDecode):
 
   def _DecodeFn(self, batch):
     ids, pad = batch
+    if self.beam_size:
+      out = gshard_decode.BeamDecodeIds(
+          self.task, self.task.theta, NestedMap(ids=ids, paddings=pad), beam_size=self.beam_size)
+      # the best hypothesis; its ids are the continuation alone, so it starts at column 0
+      return (out.topk_ids[:, 0], torch.zeros_like(out.prefix_lens), out.topk_lens[:, 0],
+              out.topk_scores[:, 0])
     out = gshard_decode.DecodeIds(
         self.task, self.task.theta, NestedMap(ids=ids, paddings=pad),
         temperature=self.temperature)
@@ -168,10 +179,12 @@ def main(argv=None):
   ap.add_argument('--max_decode_steps', type=int, default=0)
   ap.add_argument('--temperature', type=float, default=0.0)
   ap.add_argument('--params_override', default='')
+  ap.add_argument('--beam_size', type=int, default=0,
+                  help='flat beam search with this many hypotheses; 0: greedy / sampling')
   a = ap.parse_args(argv)
   dec = GShardLMDecodeBatch(a.model, a.checkpoint, a.prefix_max_len, a.batch_size,
                             a.max_decode_steps or None, a.temperature,
-                            params_override=a.params_override)
+                            params_override=a.params_override, beam_size=a.beam_size)
   dec.DecodeFiles(a.input.split(','), a.output)
   dec.stop()
   return 0

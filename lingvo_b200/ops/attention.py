@@ -228,3 +228,97 @@ def decode_attention(q, k_new, v_new, k_cache, v_cache, t, rel=None, scale=1.0):
       v_new.reshape(b, hk, d).contiguous(), k_cache, v_cache, tt.reshape(()), rel,
       float(scale))
   return out.reshape(b, 1, h, d)
+
+
+# ------------------------------------------------------------------- flat beam search ----
+def unpack_visibility(vis, n):
+  """int32 `[..., ⌈n/32⌉]` bit masks (bit j%32 of word j/32 for row j) → bool `[..., n]`."""
+  bits = (vis.unsqueeze(-1) >> torch.arange(32, device=vis.device, dtype=vis.dtype)) & 1
+  return bits.reshape(*vis.shape[:-1], -1)[..., :n].bool()
+
+
+def pack_visibility(mask):
+  """bool `[..., n]` → int32 `[..., ⌈n/32⌉]` bit masks, the inverse of `unpack_visibility`."""
+  n = mask.shape[-1]
+  w = (n + 31) // 32
+  m = F.pad(mask.to(torch.int64), (0, 32 * w - n)).reshape(*mask.shape[:-1], w, 32)
+  words = (m << torch.arange(32, device=mask.device, dtype=torch.int64)).sum(-1)
+  return torch.where(words >= 2**31, words - 2**32, words).to(torch.int32)
+
+
+def flat_beam_attention_ref(q, k_new, v_new, k_cache, v_cache, slot0, vis, qpos, kpos, rel=None,
+                            scale=1.0, logit_cap=0.0):
+  """fp32 oracle and CPU path of `flat_beam_attention`: writes row slot0 + k of the caches
+  from k_new / v_new[:, k], then takes fp32 logits over all N rows, adds the bias, applies
+  the cap (q·k + bias first, as the single-query decode step does) and drops the rows that
+  are not visible. A query that sees no row returns zeros."""
+  bsz, kh, h, d = q.shape
+  n, hk = k_cache.shape[1], k_cache.shape[2]
+  dev = q.device
+  s0 = torch.as_tensor(slot0, device=dev).reshape(()).long()
+  rows = torch.arange(n, device=dev)
+  sel = (rows.unsqueeze(0) == s0 + torch.arange(kh, device=dev).unsqueeze(1))   # [K, N]
+  written = sel.any(0).reshape(1, n, 1, 1)
+  selc = sel.to(k_cache.dtype)
+  k_cache.copy_(torch.where(written, torch.einsum('kn,bkhd->bnhd', selc, k_new.to(k_cache.dtype)),
+                            k_cache))
+  v_cache.copy_(torch.where(written, torch.einsum('kn,bkhd->bnhd', selc, v_new.to(v_cache.dtype)),
+                            v_cache))
+  g = h // hk
+  qg = q.float().reshape(bsz, kh, hk, g, d)
+  logits = torch.einsum('bkcgd,bncd->bkcgn', qg, k_cache.float()).reshape(bsz, kh, h, n)
+  logits = logits * scale
+  if rel is not None:
+    idx = (qpos.long().unsqueeze(-1) - kpos.long().unsqueeze(1) + n - 1).clamp(0, 2 * n - 2)
+    logits = logits + rel.float()[:, idx].permute(1, 2, 0, 3)                # [B,K,H,N]
+  if logit_cap:
+    logits = logit_cap * torch.tanh(logits / logit_cap)
+  live = rows < (s0 + kh).clamp(0, n)
+  visible = (unpack_visibility(vis, n) & live).unsqueeze(2)                  # [B,K,1,N]
+  logits = logits.masked_fill(~visible, float('-inf'))
+  probs = torch.softmax(logits, -1).nan_to_num(0.0)
+  vv = v_cache.float().unsqueeze(1).expand(bsz, kh, n, hk, d)
+  out = torch.einsum('bkcgn,bkncd->bkcgd', probs.reshape(bsz, kh, hk, g, n), vv)
+  return out.reshape(bsz, kh, h, d).to(q.dtype)
+
+
+def flat_beam_attention_supported(q, k_cache):
+  from lingvo_b200 import ops
+  mod = ops.native(required=False) if q.is_cuda else None
+  return (mod is not None and hasattr(mod, '_has_flat_beam_attn') and
+          ops.use_cuda_kernels(q, k_cache) and q.dtype == torch.bfloat16 and
+          k_cache.dtype == torch.bfloat16 and q.dim() == 4 and k_cache.dim() == 4 and
+          1 <= q.shape[1] <= 16 and q.shape[-1] == 128 and k_cache.shape[-1] == 128 and
+          q.shape[2] % k_cache.shape[2] == 0 and k_cache.is_contiguous())
+
+
+def flat_beam_attention(q, k_new, v_new, k_cache, v_cache, slot0, vis, qpos, kpos, rel=None,
+                        scale=1.0, logit_cap=0.0):
+  """One flat-beam-search step of self-attention: K hypotheses per sequence share one token
+  buffer (the caches), and each attends over its own set of rows.
+
+  q `[B,K,H,D]`, k_new / v_new `[B,K,Hk,D]` (Hk divides H; query head h reads KV head
+  h // (H/Hk)), caches `[B,N,Hk,D]` updated in place at rows slot0 + k, `slot0` a Python int
+  or 0-dim integer tensor. Hypothesis k sees the rows whose bit is set in the int32 mask
+  `vis[b, k]` `[B,K,⌈N/32⌉]` (see `pack_visibility`), and only rows below slot0 + K. `qpos`
+  `[B,K]` and `kpos` `[B,N]` are the positions that index the optional fp32 `[H, 2N-1]` table
+  `rel` at qpos − kpos + N − 1 (clamped to the table). Returns `[B,K,H,D]`.
+
+  On the GPU (bf16, D = 128, K ≤ 16, no `logit_cap`) this is our kernel in
+  csrc/decode_attn.cu: each K/V tile is read once for all hypotheses and query heads of a KV
+  head, only rows below slot0 + K are read, and the launch shape does not depend on slot0,
+  so a step with `slot0` as a device scalar can be captured in a CUDA graph.
+  """
+  if logit_cap or not flat_beam_attention_supported(q, k_cache):
+    return flat_beam_attention_ref(q, k_new, v_new, k_cache, v_cache, slot0, vis, qpos, kpos,
+                                   rel, scale, logit_cap)
+  from lingvo_b200 import ops
+  s0 = torch.as_tensor(slot0, device=q.device)
+  if s0.dtype not in (torch.int32, torch.int64):
+    s0 = s0.long()
+  if rel is not None:
+    rel = rel.float().contiguous()
+  return ops.native().flat_beam_attn_fwd(
+      q.contiguous(), k_new.contiguous(), v_new.contiguous(), k_cache, v_cache, s0.reshape(()),
+      vis.to(torch.int32).contiguous(), qpos.to(torch.int32).contiguous(),
+      kpos.to(torch.int32).contiguous(), rel, float(scale))

@@ -15,7 +15,21 @@ tokens, with the kernel and with `decode_attention_supported` patched to False, 
 
     python tools/decode_attn_bench.py --out DIR [--e2e-repeats 3] [--skip-e2e]
 
-Writes DIR/decode_attn_bench.json and prints one JSON line per measurement.
+With `--beam` it measures flat beam search instead:
+
+  * op level: `flat_beam_attention` (kernel) against `flat_beam_attention_ref` for
+    B ∈ {1, 8}, K ∈ {4, 8}, H = 16, Hk ∈ {16, 4, 1}, N ∈ {1024, 4096}, with slot0 = N − K and
+    ancestor-shaped masks (a 64-token prompt, then a random parent per step). Bandwidth counts
+    the live K/V rows 2·2·B·N·Hk·128, the masks and positions, q, the output and the partials.
+  * prefill: `UniTransformer.Prefill` of a P = 512 prompt against feeding the same prompt
+    through `DecodeStep` one token at a time, B = 8, on the end-to-end model below.
+  * end to end: `BeamDecodeIds` with K = 4 against greedy `DecodeIds`, B = 8, a 16-token
+    prompt and at most 256 new tokens, alternated. The model's EOS id is −1, which the beam
+    reads as the last vocabulary entry, so it may stop early on its score gap; greedy runs all
+    256 steps.
+
+Writes DIR/decode_attn_bench.json (DIR/flat_beam_bench.json with `--beam`) and prints one
+JSON line per measurement.
 """
 
 import argparse
@@ -58,9 +72,9 @@ def _TimeCalls(fn, iters, warm=5):
   return ts[len(ts) // 2]
 
 
-def _KernelDeviceUs(fn, iters):
-  """Mean device time per call of the `decode_attn_*` kernels (split + combine), from
-  `torch.profiler`, each call after an L2 flush."""
+def _KernelDeviceUs(fn, iters, name='decode_attn'):
+  """Mean device time per call of the kernels whose name contains `name` (split + combine),
+  from `torch.profiler`, each call after an L2 flush."""
   from torch.profiler import profile, ProfilerActivity   # pylint: disable=g-import-not-at-top
   flush = torch.empty(128 << 20, dtype=torch.int8, device='cuda')
   fn()
@@ -70,8 +84,8 @@ def _KernelDeviceUs(fn, iters):
       flush.zero_()
       fn()
     torch.cuda.synchronize()
-  total = sum(e.device_time_total for e in prof.key_averages() if 'decode_attn' in e.key)
-  assert total > 0, 'no decode_attn kernels in the trace'
+  total = sum(e.device_time_total for e in prof.key_averages() if name in e.key)
+  assert total > 0, 'no %s kernels in the trace' % name
   return total / iters
 
 
@@ -185,21 +199,156 @@ def _EndToEnd(records, repeats):
   records.append(rec)
 
 
+# ------------------------------------------------------------------- flat beam search ----
+def _AncestorVis(b, kk, n, slot0, prompt=64, seed=0):
+  g = torch.Generator().manual_seed(seed)
+  mask = torch.zeros(b, kk, n, dtype=torch.bool)
+  mask[:, :, :prompt] = True
+  for s0 in range(prompt, slot0, kk):
+    mask[:, torch.arange(kk), s0 + torch.arange(kk)] = True
+    parent = torch.randint(0, kk, (b, kk), generator=g)
+    mask = mask.gather(1, parent.unsqueeze(-1).expand(b, kk, n))
+  mask[:, torch.arange(kk), slot0 + torch.arange(kk)] = True
+  return attention_ops.pack_visibility(mask).cuda()
+
+
+def _BeamOpLevel(records):
+  nat = ops.native()
+  h = 16
+  for b in (1, 8):
+    for n in (1024, 4096):
+      for kk in (4, 8):
+        vis = _AncestorVis(b, kk, n, n - kk)
+        for hk in (16, 4, 1):
+          g = torch.Generator(device='cuda').manual_seed(0)
+          ck = torch.randn(b, n, hk, 128, generator=g, device='cuda').to(torch.bfloat16)
+          cv = torch.randn(b, n, hk, 128, generator=g, device='cuda').to(torch.bfloat16)
+          q = (torch.randn(b, kk, h, 128, generator=g, device='cuda') * 0.1).to(torch.bfloat16)
+          kn = torch.randn(b, kk, hk, 128, generator=g, device='cuda').to(torch.bfloat16)
+          vn = torch.randn(b, kk, hk, 128, generator=g, device='cuda').to(torch.bfloat16)
+          rel = torch.randn(h, 2 * n - 1, generator=g, device='cuda')
+          qpos = torch.full((b, kk), n - 1, dtype=torch.int32, device='cuda')
+          kpos = torch.arange(n, dtype=torch.int32, device='cuda').repeat(b, 1)
+          s0 = torch.tensor(n - kk, device='cuda')
+          chunk = nat.flat_beam_attn_chunk(b, kk, h, hk, n)
+          splits = (n + chunk - 1) // chunk
+          args = (q, kn, vn, ck, cv, s0, vis, qpos, kpos, rel)
+          kern = lambda: attention_ops.flat_beam_attention(*args)  # pylint: disable=cell-var-from-loop
+          ref = lambda: attention_ops.flat_beam_attention_ref(*args)  # pylint: disable=cell-var-from-loop
+          err = float((kern().float() - ref().float()).norm() / ref().float().norm())
+          call_k = _TimeCalls(kern, 200)
+          us_r = _TimeCalls(ref, 20)
+          us_k = _KernelDeviceUs(kern, 100, 'flat_beam_attn')
+          nbytes = (2 * 2 * b * n * hk * 128 + b * kk * ((n + 31) // 32) * 4 + b * n * 4 +
+                    2 * b * kk * h * 128 * 2 +
+                    (2 * b * kk * h * splits * (128 + 2) * 4 if splits > 1 else 0))
+          rec = dict(kind='beam_op', B=b, K=kk, N=n, slot0=n - kk, H=h, Hk=hk, chunk=chunk,
+                     splits=splits, kernel_us=us_k, kernel_call_us=call_k, ref_call_us=us_r,
+                     speedup_per_call=us_r / call_k, kernel_bytes=nbytes,
+                     kernel_GBps=nbytes / us_k / 1e3,
+                     kernel_share_of_3p35TBps=nbytes / (us_k * 1e-6) / HBM_BYTES_PER_S,
+                     kernel_peak_bytes=_PeakBytes(kern), ref_peak_bytes=_PeakBytes(ref),
+                     rel_err_vs_ref=err)
+          print(json.dumps(rec))
+          sys.stdout.flush()
+          records.append(rec)
+          del ck, cv
+          torch.cuda.empty_cache()
+
+
+def _Timed(fn):
+  torch.cuda.synchronize()
+  t0 = time.perf_counter()
+  out = fn()
+  torch.cuda.synchronize()
+  return time.perf_counter() - t0, out
+
+
+def _BeamPrefill(records, task, repeats):
+  b, plen = 8, 512
+  ids = torch.randint(2, 32000, (b, plen), device='cuda')
+  seg = torch.ones(b, plen, dtype=torch.long, device='cuda')
+  pos = torch.arange(plen, device='cuda').repeat(b, 1)
+
+  def Prefill():
+    st = task.InitDecodeState(b, plen, ids.device)
+    task.Prefill(task.theta, ids, seg, pos, st)
+    return st
+
+  def Teacher():
+    st = task.InitDecodeState(b, plen, ids.device)
+    for t in range(plen):
+      task.DecodeStep(task.theta, ids[:, t], st, t)
+    return st
+
+  with torch.no_grad():
+    a, c = Prefill(), Teacher()
+    err = max(float((x.k.float() - y.k.float()).norm() / y.k.float().norm())
+              for x, y in zip(a, c) if x is not None)
+    times = {'prefill': [], 'decode_steps': []}
+    for _ in range(repeats):
+      times['prefill'].append(_Timed(Prefill)[0])
+      times['decode_steps'].append(_Timed(Teacher)[0])
+  rec = dict(kind='beam_prefill', B=b, P=plen, prefill_s=times['prefill'],
+             decode_steps_s=times['decode_steps'],
+             speedup=min(times['decode_steps']) / min(times['prefill']),
+             cache_rel_err_vs_decode_steps=err)
+  print(json.dumps(rec))
+  records.append(rec)
+
+
+def _BeamEndToEnd(records, task, repeats):
+  from lingvo_b200.core import gshard_decode   # pylint: disable=g-import-not-at-top
+  from lingvo_b200.core.nested_map import NestedMap   # pylint: disable=g-import-not-at-top
+  b, prefix, steps, kk = 8, 16, 256, 4
+  ids = torch.randint(2, 32000, (b, prefix), device='cuda')
+  batch = NestedMap(ids=ids, labels=ids, paddings=torch.zeros(b, prefix, device='cuda'))
+  run = {
+      'beam': lambda: gshard_decode.BeamDecodeIds(task, task.theta, batch, beam_size=kk,
+                                                  max_steps=steps),
+      'greedy': lambda: gshard_decode.DecodeIds(task, task.theta, batch, max_steps=steps),
+  }
+  with torch.no_grad():
+    for fn in run.values():
+      fn()
+    times = {k: [] for k in run}
+    for _ in range(repeats):
+      for k, fn in run.items():
+        times[k].append(_Timed(fn)[0])
+  rec = dict(kind='beam_e2e', B=b, K=kk, prefix=prefix, new_tokens=steps, layers=8,
+             model_dim=2048, heads='16x128', beam_s=times['beam'], greedy_s=times['greedy'],
+             beam_over_greedy=min(times['beam']) / min(times['greedy']),
+             beam_hyp_tokens_per_s=b * kk * steps / min(times['beam']),
+             greedy_tokens_per_s=b * steps / min(times['greedy']))
+  print(json.dumps(rec))
+  records.append(rec)
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--out', required=True, help='output directory')
   ap.add_argument('--e2e-repeats', type=int, default=3)
   ap.add_argument('--skip-e2e', action='store_true')
+  ap.add_argument('--beam', action='store_true', help='measure flat beam search')
   args = ap.parse_args()
   assert torch.cuda.is_available(), 'decode_attn_bench needs a GPU'
   ops.native(required=True)
   os.makedirs(args.out, exist_ok=True)
   records = [dict(kind='card', **_Card())]
   print(json.dumps(records[0]))
-  _OpLevel(records)
-  if not args.skip_e2e:
-    _EndToEnd(records, args.e2e_repeats)
-  with open(os.path.join(args.out, 'decode_attn_bench.json'), 'w') as f:
+  if args.beam:
+    _BeamOpLevel(records)
+    if not args.skip_e2e:
+      torch.manual_seed(0)
+      task = _Lm()
+      _BeamPrefill(records, task, args.e2e_repeats)
+      _BeamEndToEnd(records, task, args.e2e_repeats)
+  else:
+    _OpLevel(records)
+    if not args.skip_e2e:
+      _EndToEnd(records, args.e2e_repeats)
+  name = 'flat_beam_bench.json' if args.beam else 'decode_attn_bench.json'
+  with open(os.path.join(args.out, name), 'w') as f:
     json.dump(records, f, indent=1)
 
 
