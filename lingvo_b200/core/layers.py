@@ -1854,7 +1854,8 @@ class LayerNorm(base_layer.BaseLayer):
   """Layer normalisation (reference :4927).
 
   scale stored as `(1 + scale)` unless `direct_scale`; `bias`/`center`
-  switches. On CUDA the fused sm_90a kernel (`ops.norm.layer_norm`) is used.
+  switches. bf16 inputs on CUDA take the fused sm_90a kernel (`ops.norm.layer_norm`);
+  every other input is normalised in fp32 and keeps its dtype.
   """
 
   @classmethod
@@ -1898,7 +1899,8 @@ class LayerNorm(base_layer.BaseLayer):
     p = self.params
     inputs = self._CastToFPropDtype(inputs)
     scale, bias = self._GetScaleAndBias(theta)
-    if ops.use_cuda_kernels(inputs) and inputs.shape[-1] % 8 == 0:
+    if (inputs.dtype == torch.bfloat16 and ops.use_cuda_kernels(inputs) and
+        inputs.shape[-1] % 8 == 0):
       from lingvo_b200.ops import norm
       if norm.available():
         return norm.layer_norm(inputs, scale, bias, p.epsilon, center=p.center)

@@ -37,6 +37,8 @@ class _GluDwConvFn(torch.autograd.Function):
 
 
 def glu_dwconv1d_supported(x, conv_layer):
+  """True when the fused kernel serves this depthwise conv layer. Kernel sizes above the
+  backward's shared-memory limit (`glu_dwconv_max_k`) take the unfused path."""
   p = conv_layer.params
   import os  # pylint: disable=g-import-not-at-top
   if os.environ.get('LINGVO_B200_DISABLE_FUSED_CONV') == '1':   # A/B switch for benchmarks
@@ -46,7 +48,8 @@ def glu_dwconv1d_supported(x, conv_layer):
                                         'CausalDepthwiseConv2DLayer') and
           p.filter_shape[1] == 1 and p.filter_shape[3] == 1 and
           tuple(p.filter_stride) == (1, 1) and tuple(p.dilation_rate) == (1, 1) and
-          not p.bias and not p.partial_conv and p.filter_shape[0] <= 128)
+          not p.bias and not p.partial_conv and
+          p.filter_shape[0] <= ops.native().glu_dwconv_max_k)
 
 
 def glu_dwconv1d(proj, w, paddings, causal=False):

@@ -336,6 +336,20 @@ norm_bwd_fold_kernel(const float* __restrict__ part_s, const float* __restrict__
   }
 }
 
+bool Aligned16(const torch::Tensor& t) {
+  return reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0;
+}
+
+// scale / bias as the fp32 [dim] vector the kernels read with 16-byte loads.
+torch::Tensor ParamVector(const torch::Tensor& v, const torch::Tensor& x, int dim,
+                          const char* name) {
+  TORCH_CHECK(v.device() == x.device() && v.numel() == dim, "norm: ", name, " must have ", dim,
+              " elements on x's device, got ", v.numel());
+  auto f = v.to(torch::kFloat32).contiguous();
+  TORCH_CHECK(Aligned16(f), "norm: ", name, " must be 16-byte aligned");
+  return f;
+}
+
 int GridFor(int rows) {
   const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
   int ctas = (rows + kWarpsPerCta - 1) / kWarpsPerCta;
@@ -349,24 +363,29 @@ std::vector<torch::Tensor> norm_fwd(const torch::Tensor& x, const c10::optional<
                                     const c10::optional<torch::Tensor>& scale,
                                     const c10::optional<torch::Tensor>& bias, double eps,
                                     bool center, bool write_sum) {
-  TORCH_CHECK(x.is_cuda() && x.scalar_type() == torch::kBFloat16 && x.is_contiguous());
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == torch::kBFloat16 && x.is_contiguous(),
+              "norm: x must be a contiguous CUDA bf16 tensor");
+  const int dim = x.dim() > 0 ? static_cast<int>(x.size(-1)) : 0;
+  TORCH_CHECK(dim > 0 && dim % 8 == 0, "norm: last dim must be a positive multiple of 8");
+  TORCH_CHECK(Aligned16(x), "norm: x must be 16-byte aligned");
+  const bool has_res = res.has_value() && res->defined();
+  if (has_res)
+    TORCH_CHECK(res->device() == x.device() && res->scalar_type() == torch::kBFloat16 &&
+                res->is_contiguous() && res->numel() == x.numel() && Aligned16(*res),
+                "norm: res must be a contiguous 16-byte-aligned bf16 tensor like x");
+  torch::Tensor sc, bi;
+  if (scale.has_value() && scale->defined()) sc = ParamVector(*scale, x, dim, "scale");
+  if (bias.has_value() && bias->defined()) bi = ParamVector(*bias, x, dim, "bias");
   const c10::cuda::CUDAGuard guard(x.device());
-  const int dim = static_cast<int>(x.size(-1));
-  TORCH_CHECK(dim % 8 == 0, "norm: last dim must be a multiple of 8");
   const int rows = static_cast<int>(x.numel() / dim);
   auto y = torch::empty_like(x);
   auto stats = torch::empty({rows, 2}, x.options().dtype(torch::kFloat32));
   torch::Tensor sum;
   const __nv_bfloat16* rp = nullptr;
-  if (res.has_value() && res->defined()) {
-    TORCH_CHECK(res->scalar_type() == torch::kBFloat16 && res->is_contiguous() &&
-                res->numel() == x.numel());
+  if (has_res) {
     rp = reinterpret_cast<const __nv_bfloat16*>(res->data_ptr());
     if (write_sum) sum = torch::empty_like(x);
   }
-  torch::Tensor sc, bi;
-  if (scale.has_value() && scale->defined()) sc = scale->to(torch::kFloat32).contiguous();
-  if (bias.has_value() && bias->defined()) bi = bias->to(torch::kFloat32).contiguous();
   if (rows == 0) return {y, stats, sum.defined() ? sum : torch::Tensor()};
   auto stream = at::cuda::getCurrentCUDAStream();
   const int grid = GridFor(rows);
@@ -393,13 +412,27 @@ std::vector<torch::Tensor> norm_bwd(const torch::Tensor& x, const torch::Tensor&
                                     const c10::optional<torch::Tensor>& scale,
                                     const torch::Tensor& stats, bool center, bool need_dscale,
                                     bool need_dbias) {
-  TORCH_CHECK(x.is_cuda() && dy.is_cuda() && x.is_contiguous() && dy.is_contiguous());
-  const c10::cuda::CUDAGuard guard(x.device());
-  const int dim = static_cast<int>(x.size(-1));
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == torch::kBFloat16 && x.is_contiguous(),
+              "norm_bwd: x must be a contiguous CUDA bf16 tensor");
+  const int dim = x.dim() > 0 ? static_cast<int>(x.size(-1)) : 0;
+  TORCH_CHECK(dim > 0 && dim % 8 == 0, "norm_bwd: last dim must be a positive multiple of 8");
+  TORCH_CHECK(dy.device() == x.device() && dy.scalar_type() == torch::kBFloat16 &&
+              dy.is_contiguous() && dy.sizes() == x.sizes(),
+              "norm_bwd: dy must be a contiguous bf16 tensor of x's shape");
+  TORCH_CHECK(Aligned16(x) && Aligned16(dy), "norm_bwd: x and dy must be 16-byte aligned");
   const int rows = static_cast<int>(x.numel() / dim);
-  auto dx = torch::empty_like(x);
+  TORCH_CHECK(stats.device() == x.device() && stats.scalar_type() == torch::kFloat32 &&
+              stats.is_contiguous() && stats.dim() == 2 && stats.size(0) == rows &&
+              stats.size(1) == 2, "norm_bwd: stats must be contiguous fp32 [rows, 2]");
+  const bool has_dres = dres.has_value() && dres->defined();
+  if (has_dres)
+    TORCH_CHECK(dres->device() == x.device() && dres->scalar_type() == torch::kBFloat16 &&
+                dres->is_contiguous() && dres->numel() == x.numel() && Aligned16(*dres),
+                "norm_bwd: dres must be a contiguous 16-byte-aligned bf16 tensor like x");
   torch::Tensor sc, ds, db;
-  if (scale.has_value() && scale->defined()) sc = scale->to(torch::kFloat32).contiguous();
+  if (scale.has_value() && scale->defined()) sc = ParamVector(*scale, x, dim, "scale");
+  const c10::cuda::CUDAGuard guard(x.device());
+  auto dx = torch::empty_like(x);
   if (need_dscale) ds = torch::empty({dim}, x.options().dtype(torch::kFloat32));
   if (need_dbias) db = torch::empty({dim}, x.options().dtype(torch::kFloat32));
   if (rows == 0) {
@@ -407,11 +440,8 @@ std::vector<torch::Tensor> norm_bwd(const torch::Tensor& x, const torch::Tensor&
     if (db.defined()) db.zero_();
     return {dx, ds, db};
   }
-  const __nv_bfloat16* drp = nullptr;
-  if (dres.has_value() && dres->defined()) {
-    TORCH_CHECK(dres->is_contiguous() && dres->scalar_type() == torch::kBFloat16);
-    drp = reinterpret_cast<const __nv_bfloat16*>(dres->data_ptr());
-  }
+  const __nv_bfloat16* drp =
+      has_dres ? reinterpret_cast<const __nv_bfloat16*>(dres->data_ptr()) : nullptr;
   auto stream = at::cuda::getCurrentCUDAStream();
   // dx: one light streaming kernel (48 registers, no parameter-gradient work) on a persistent
   // grid; dscale / dbias: column-reduction kernel + fold.

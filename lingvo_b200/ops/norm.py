@@ -89,9 +89,12 @@ def rms_norm_pass(x, scale, eps):
 
 
 def layer_norm(x, scale, bias, eps, center=True):
-  if x.dtype != torch.bfloat16:
-    x = x.to(torch.bfloat16)
-  return _NormFn.apply(x, scale, bias if center else None, float(eps), center)
+  """bf16 x → bf16 LayerNorm (center=False: no mean subtraction, as RMS norm). The bias is
+  added whether or not the norm centres; without centring it is added outside the kernel."""
+  if center:
+    return _NormFn.apply(x, scale, bias, float(eps), True)
+  y = _NormFn.apply(x, scale, None, float(eps), False)
+  return y if bias is None else (y.float() + bias.float()).to(y.dtype)
 
 
 def rms_norm_ref(x, scale, eps):
