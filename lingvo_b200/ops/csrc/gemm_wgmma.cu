@@ -596,6 +596,7 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
   const int64_t N = b_kmajor ? b.size(1) : b.size(2);
   const int64_t Kb = b_kmajor ? b.size(2) : b.size(1);
   TORCH_CHECK(K == Kb, "gemm_bf16: K mismatch ", K, " vs ", Kb);
+  TORCH_CHECK(K > 0, "gemm_bf16: K must be positive, got K = ", K);
   TORCH_CHECK(N % 8 == 0, "gemm_bf16: N must be a multiple of 8");
   auto check_op = [](const torch::Tensor& t) {
     TORCH_CHECK(t.stride(1) % 8 == 0 && (t.size(0) == 1 || t.stride(0) % 8 == 0) &&
@@ -639,6 +640,10 @@ torch::Tensor gemm_bf16(const torch::Tensor& a_in, const torch::Tensor& b_in, bo
   if (has_aux) {
     torch::Tensor ax = aux.value();
     ax = ax.dim() == 2 ? ax.unsqueeze(0) : ax;
+    // The aux tensor map takes out's sizes, so a smaller aux would be read past its end.
+    TORCH_CHECK(ax.dim() == 3 && ax.size(0) == G && ax.size(1) == M && ax.size(2) == N,
+                "gemm_bf16: aux must have out's sizes [G, M, N] = [", G, ", ", M, ", ", N,
+                "] (2-D only with G = 1), got ", ax.sizes());
     TORCH_CHECK(ax.scalar_type() == torch::kBFloat16 && ax.stride(1) == p.ldc &&
                     (G == 1 || ax.stride(0) == p.c_batch) && ax.stride(2) == 1,
                 "gemm_bf16: aux must be bf16 with the same strides as out");
