@@ -168,8 +168,9 @@ def flash_attention(q, k, v, rel=None, seg=None, pos=None, scale=1.0, causal=Fal
 # ------------------------------------------------------- incremental decoding ----
 def decode_attention_ref(q, k_new, v_new, k_cache, v_cache, t, rel=None, scale=1.0):
   """fp32 oracle and CPU path of `decode_attention`: one-hot write of row t into the caches,
-  fp32 logits over all T keys, −1e9 on the keys after t. Grouped / multi-query KV heads are
-  expanded with `_ExpandKv`."""
+  fp32 logits over all T keys, −1e9 on the keys after t when t is in [0, T) (otherwise every
+  key is visible, as in the kernel). Grouped / multi-query KV heads are expanded with
+  `_ExpandKv`."""
   bsz, _, h, _ = q.shape
   tmax = k_cache.shape[1]
   dev = q.device
@@ -185,7 +186,8 @@ def decode_attention_ref(q, k_new, v_new, k_cache, v_cache, t, rel=None, scale=1
   if rel is not None:
     idx = (tt - key_pos + tmax - 1).clamp(0, 2 * tmax - 2)
     logits = logits + rel.float()[:, idx].reshape(1, h, 1, tmax)
-  logits = logits + ((key_pos > tt).float() * -1e9).reshape(1, 1, 1, tmax)
+  masked = (key_pos > tt) & (tt >= 0) & (tt < tmax)
+  logits = logits + (masked.float() * -1e9).reshape(1, 1, 1, tmax)
   probs = torch.softmax(logits, -1)
   return torch.einsum('bhqk,bkhd->bqhd', probs, vv.float()).to(q.dtype)
 

@@ -61,17 +61,21 @@ def init_state(num_beams, num_hyps_per_beam, max_steps, src_len, device,
 
 
 def _TopKRef(log_probs, cum, active, k, eos_id):
-  """Plain-PyTorch form of `beam_topk` (CPU path and numerics oracle of the kernel)."""
+  """Plain-PyTorch form of `beam_topk` (CPU path and numerics oracle of the kernel).
+
+  Scores are floored at NEG as in the kernel, whose lists start at NEG: a row with fewer than
+  k candidates above NEG pads its top-k with (NEG, word 0), and a row whose every score is
+  below NEG has best_in_hyp = NEG."""
   lp = log_probs.float()
   glob = cum.unsqueeze(1) + lp
-  best_in_hyp = glob.max(1).values
+  best_in_hyp = glob.max(1).values.clamp_min(NEG)
   eos_glob = glob[:, eos_id]
   glob_no_eos = glob.clone()
   glob_no_eos[:, eos_id] = NEG
   glob_no_eos = torch.where(active.unsqueeze(1), glob_no_eos, torch.full_like(glob_no_eos, NEG))
   # score desc, word id asc on ties: stable sort of the (ascending-id) row
   order = torch.argsort(glob_no_eos, dim=1, descending=True, stable=True)[:, :k]
-  top_s = glob_no_eos.gather(1, order)
+  top_s = glob_no_eos.gather(1, order).clamp_min(NEG)
   top_w = torch.where(top_s > NEG / 2, order, torch.zeros_like(order))
   return top_s, top_w, best_in_hyp, eos_glob, lp[:, eos_id]
 
