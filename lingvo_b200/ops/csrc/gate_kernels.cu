@@ -231,12 +231,21 @@ gate_logits_dgw_fold_kernel(const float* __restrict__ part, WT* __restrict__ dgw
 
 int Sms() { return at::cuda::getCurrentDeviceProperties()->multiProcessorCount; }
 
+bool Aligned16(const torch::Tensor& t) {
+  return reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0;
+}
+
+// x and dres are read with 16-byte `ld.global.nc.v4` loads (gate_load8).
 void CheckArgs(const torch::Tensor& x, const torch::Tensor& gw) {
   TORCH_CHECK(x.is_cuda() && x.scalar_type() == torch::kBFloat16 && x.is_contiguous() && x.dim() == 2,
               "gate_logits: x must be contiguous bf16 [T, M]");
+  TORCH_CHECK(Aligned16(x), "gate_logits: x must be 16-byte aligned");
   TORCH_CHECK(gw.is_cuda() && gw.is_contiguous() && gw.dim() == 2 && gw.size(0) == x.size(1),
               "gate_logits: gw must be contiguous [M, E]");
+  TORCH_CHECK(gw.device() == x.device(), "gate_logits: gw must be on x's device");
   TORCH_CHECK(gw.scalar_type() == torch::kFloat32 || gw.scalar_type() == torch::kBFloat16);
+  const int64_t e = gw.size(1);
+  TORCH_CHECK(e == 2 || e == 4 || e == 8 || e == 16, "gate_logits: unsupported expert count ", e);
   TORCH_CHECK(x.size(1) % 8 == 0, "gate_logits: M must be a multiple of 8");
   TORCH_CHECK(static_cast<size_t>(x.size(1)) * gw.size(1) * 4 <= 200 * 1024,
               "gate_logits: [M, E] weight does not fit in shared memory");
@@ -300,6 +309,7 @@ std::vector<torch::Tensor> gate_logits_bwd(const torch::Tensor& x, const torch::
   TORCH_CHECK(dlogits.is_cuda() && dlogits.scalar_type() == torch::kFloat32 &&
               dlogits.is_contiguous() && dlogits.dim() == 2 && dlogits.size(0) == x.size(0) &&
               dlogits.size(1) == gw.size(1), "gate_logits_bwd: dlogits must be fp32 [T, E]");
+  TORCH_CHECK(dlogits.device() == x.device(), "gate_logits_bwd: dlogits must be on x's device");
   const c10::cuda::CUDAGuard guard(x.device());
   const int T = static_cast<int>(x.size(0)), M = static_cast<int>(x.size(1));
   const int64_t E = gw.size(1);
@@ -310,6 +320,8 @@ std::vector<torch::Tensor> gate_logits_bwd(const torch::Tensor& x, const torch::
   if (dres.has_value() && dres->defined()) {
     TORCH_CHECK(dres->is_cuda() && dres->scalar_type() == torch::kBFloat16 && dres->is_contiguous() &&
                 dres->numel() == x.numel(), "gate_logits_bwd: dres must be contiguous bf16 like x");
+    TORCH_CHECK(dres->device() == x.device(), "gate_logits_bwd: dres must be on x's device");
+    TORCH_CHECK(Aligned16(*dres), "gate_logits_bwd: dres must be 16-byte aligned");
     drp = reinterpret_cast<const __nv_bfloat16*>(dres->data_ptr());
   }
   if (need_dx) {

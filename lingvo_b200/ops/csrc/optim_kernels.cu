@@ -25,6 +25,7 @@
 #include <mutex>
 #include <utility>
 
+#include "adam.cuh"
 #include "ptx.cuh"
 #include "registry.h"
 
@@ -410,12 +411,7 @@ __global__ void adam_flat_kernel(float* __restrict__ w, const GT* __restrict__ g
     load_g8<float>(m + i, mf);
     load_g8<float>(v + i, vf);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const float gg = gf[k] * gs;
-      mf[k] = b1 * mf[k] + (1.f - b1) * gg;
-      vf[k] = b2 * vf[k] + (1.f - b2) * gg * gg;
-      wf[k] -= lr_t * mf[k] / (sqrtf(vf[k]) + eps);
-    }
+    for (int k = 0; k < 8; ++k) adam_update(wf[k], mf[k], vf[k], gf[k] * gs, lr_t, b1, b2, eps);
     *reinterpret_cast<float4*>(w + i) = make_float4(wf[0], wf[1], wf[2], wf[3]);
     *reinterpret_cast<float4*>(w + i + 4) = make_float4(wf[4], wf[5], wf[6], wf[7]);
     *reinterpret_cast<float4*>(m + i) = make_float4(mf[0], mf[1], mf[2], mf[3]);

@@ -17,7 +17,10 @@ def available() -> bool:
 
 
 def supported(x, gw) -> bool:
+  """The kernels read x with 16-byte loads, so a contiguous x must start 16-byte aligned (a
+  strided x is copied first)."""
   return (available() and x.is_cuda and x.dtype == torch.bfloat16 and gw.is_cuda and
+          gw.device == x.device and (x.data_ptr() % 16 == 0 or not x.is_contiguous()) and
           gw.dtype in (torch.float32, torch.bfloat16) and gw.dim() == 2 and
           gw.shape[1] in _SUPPORTED_E and x.shape[-1] == gw.shape[0] and
           gw.shape[0] % 8 == 0 and gw.shape[0] * gw.shape[1] * 4 <= 200 * 1024)
@@ -57,6 +60,7 @@ class _GateLogitsPassFn(torch.autograd.Function):
     gwc = gw if gw.is_contiguous() else gw.contiguous()
     ctx.save_for_backward(x2, gwc)
     ctx.x_shape = x.shape
+    ctx.set_materialize_grads(False)   # an unused output's gradient arrives as None
     out = ops.native().gate_logits_fwd(x2, gwc)
     return out.reshape(*x.shape[:-1], gw.shape[1]), x.view_as(x)
 
@@ -73,6 +77,8 @@ class _GateLogitsPassFn(torch.autograd.Function):
       dres = dres if dres.is_contiguous() else dres.contiguous()
       if dres.dtype != torch.bfloat16:
         dres = dres.to(torch.bfloat16)
+      if dres.data_ptr() % 16:
+        dres = dres.clone()            # the kernel reads dres with 16-byte loads
     dx, dgw = ops.native().gate_logits_bwd(x2, gw, dl, ctx.needs_input_grad[0],
                                            ctx.needs_input_grad[1], dres)
     return (dx.reshape(ctx.x_shape) if dx is not None else None), dgw
