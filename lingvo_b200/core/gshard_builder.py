@@ -21,7 +21,6 @@ experiment configs port 1:1.
 from __future__ import annotations
 
 import math
-import os
 from typing import List, Optional
 
 import numpy as np
@@ -48,10 +47,6 @@ def ShardedWeightParams(shape, init=None, dtype=None, collections=None,
                         tensor_split_dims_mapping=None, device_mesh=None):
   return WeightParams(shape, init, dtype, collections, device_mesh,
                       tensor_split_dims_mapping)
-
-
-# Pass-through autograd nodes that fuse gradient adds into backward kernels (A/B switch).
-_FUSE_PASS = os.environ.get('LINGVO_B200_FUSE_PASS', '1') != '0'
 
 
 def _Act(name: str):
@@ -153,11 +148,10 @@ class RmsNormLayer(_BuilderLayer):
     so `x_pass + f(norm(x))` back-propagates with the residual-gradient add fused into the
     norm backward kernel (ops/norm.py `_NormPassFn`). Falls back to (FProp(x), x)."""
     p = self.params
-    if (p.kind == 'rms' and _FUSE_PASS and ops.use_cuda_kernels(x) and
-        x.dtype == torch.bfloat16 and x.requires_grad):
+    if (p.kind == 'rms' and ops.use_cuda_kernels(x) and x.dtype == torch.bfloat16 and
+        x.requires_grad):
       from lingvo_b200.ops import norm
-      if norm.available():
-        return norm.rms_norm_pass(x, None if p.no_scale else theta.scale, p.epsilon)
+      return norm.rms_norm_pass(x, None if p.no_scale else theta.scale, p.epsilon)
     return self.FProp(theta, x), x
 
   def FProp(self, theta, x):
@@ -168,8 +162,7 @@ class RmsNormLayer(_BuilderLayer):
       scale = None if p.no_scale else theta.scale
       if ops.use_cuda_kernels(x) and x.dtype == torch.bfloat16:
         from lingvo_b200.ops import norm
-        if norm.available():
-          return norm.rms_norm(x, scale, p.epsilon)
+        return norm.rms_norm(x, scale, p.epsilon)
       xf = x.float()
       y = xf * torch.rsqrt(xf.square().mean(-1, keepdim=True) + p.epsilon)
       if scale is not None:
@@ -1061,9 +1054,8 @@ class MoELayer(_BuilderLayer):
             b.moe_hidden_dim % 8 == 0 and not (b.moe_dropout_rate and
                                               not self.do_eval)):
       return None
-    from lingvo_b200.ops import moe as moe_ops
     from lingvo_b200.parallel import mesh as mesh_lib
-    if not moe_ops.available() or mesh_lib.Get().mode != 'fused':
+    if mesh_lib.Get().mode != 'fused':
       return None
     if self._ep is not None:
       return self._ep.GetExchange(x.device)
@@ -1101,7 +1093,7 @@ class MoELayer(_BuilderLayer):
     # streaming kernel reads the bf16 activations directly (no fp32 upcast, no N=8 SGEMM).
     from lingvo_b200.ops import gate as gate_ops
     if ldt == torch.float32 and gate_ops.supported(xg, theta.gw):
-      if xg.requires_grad and _FUSE_PASS:
+      if xg.requires_grad:
         # x also feeds the expert exchange: take it from the router's autograd node so the
         # two input gradients are summed inside the router's dx kernel.
         logits, xg = gate_ops.gate_logits_pass(xg, theta.gw)
@@ -1989,10 +1981,9 @@ class UniTransformer(base_model.BaseTask):
         and p.logits_abs_max is None and not p.softmax_logit_cap and
         not p.softmax_bias):
       from lingvo_b200.ops import xent as xent_ops
-      if xent_ops.available():
-        stats = xent_ops.lm_head_xent(
-            x.reshape(-1, x.shape[-1]), theta.dec_emb.embedding.to(x.dtype),
-            labels.reshape(-1), p.label_smoothing, p.z_loss)
+      stats = xent_ops.lm_head_xent(
+          x.reshape(-1, x.shape[-1]), theta.dec_emb.embedding.to(x.dtype),
+          labels.reshape(-1), p.label_smoothing, p.z_loss)
     if stats is None:
       logits = self._ComputeLogits(theta, x).float()
       lse = torch.logsumexp(logits, -1)

@@ -1437,9 +1437,8 @@ class SimpleFullSoftmax(SoftmaxLayer):
           inputs.dtype == torch.bfloat16 and p.logits_abs_max is None and
           not p.logits_soft_max and not p.label_smoothing):
         from lingvo_b200.ops import xent as xent_ops
-        if xent_ops.available():
-          w, b = self._ConcatWeights(theta)
-          fused = xent_ops.linear_xent(inputs, w, b, class_ids.reshape(-1))
+        w, b = self._ConcatWeights(theta)
+        fused = xent_ops.linear_xent(inputs, w, b, class_ids.reshape(-1))
       if fused is not None:
         per_example_xent, per_example_argmax, logits = fused
       else:
@@ -1902,8 +1901,7 @@ class LayerNorm(base_layer.BaseLayer):
     if (inputs.dtype == torch.bfloat16 and ops.use_cuda_kernels(inputs) and
         inputs.shape[-1] % 8 == 0):
       from lingvo_b200.ops import norm
-      if norm.available():
-        return norm.layer_norm(inputs, scale, bias, p.epsilon, center=p.center)
+      return norm.layer_norm(inputs, scale, bias, p.epsilon, center=p.center)
     x = inputs.float()
     if p.center:
       mean = x.mean(-1, keepdim=True)

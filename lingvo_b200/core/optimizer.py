@@ -18,14 +18,13 @@ multi-tensor (`torch._foreach_*`) launches or as the fused sm_90a kernels in
 from __future__ import annotations
 
 import contextlib
-import os
-
 import math
 import re
 from typing import Dict, List, Optional, Tuple
 
 import torch
 
+from lingvo_b200 import ops
 from lingvo_b200.core import base_layer
 from lingvo_b200.core import py_utils
 from lingvo_b200.core.nested_map import NestedMap
@@ -385,15 +384,14 @@ class Adam(Base):
     lr_t = float(lr) * math.sqrt(1 - b2p) / (1 - b1p)
     ms = [self._Slot(v, 'm') for v in variables]
     vs = [self._Slot(v, 'v') for v in variables]
-    if p.fused and variables[0].is_cuda:
+    if p.fused and ops.use_cuda_kernels(variables[0]):
       from lingvo_b200.ops import optim
-      if optim.available():
-        optim.multi_tensor_adam(variables, grads, ms, vs, lr_t, p.beta1,
-                                p.beta2, p.epsilon,
-                                grad_scale_t=self._grad_scale)
-        for v in variables:
-          self._refreshed.add(id(v))
-        return
+      optim.multi_tensor_adam(variables, grads, ms, vs, lr_t, p.beta1,
+                              p.beta2, p.epsilon,
+                              grad_scale_t=self._grad_scale)
+      for v in variables:
+        self._refreshed.add(id(v))
+      return
     if getattr(self, '_grad_scale', None) is not None:
       gs = self._grad_scale
       grads = [torch.where(gs == 0, torch.zeros_like(g), g * gs.to(g.dtype))
@@ -624,7 +622,7 @@ class XLAShardingAdafactor(Base):
       self._used.clear()
 
   def _UpdateFan(self, device):
-    n = int(os.environ.get('LINGVO_B200_ADAFACTOR_STREAMS', self.params.num_update_streams or 0))
+    n = int(self.params.num_update_streams or 0)
     if n <= 1 or device.type != 'cuda':
       return self._Fan([])
     if getattr(self, '_side_streams', None) is None:
@@ -648,12 +646,10 @@ class XLAShardingAdafactor(Base):
     t = t + 1.0
     return p.beta2 * (1.0 - p.beta2**(t - 1.0)) / (1.0 - p.beta2**t)
 
-  def _FusedModule(self, device_is_cuda):
-    p = self.params
-    if p.fused and device_is_cuda:
+  def _FusedModule(self, var):
+    if self.params.fused and ops.use_cuda_kernels(var):
       from lingvo_b200.ops import optim
-      if optim.available():
-        return optim
+      return optim
     return None
 
   def _FusedEligible(self, var, dims):
@@ -679,9 +675,7 @@ class XLAShardingAdafactor(Base):
     Returns (device scalar Σg² over the handled variables, set of handled var ids)."""
     p = self.params
     self._pre = {}
-    if not var_grad_pairs or not var_grad_pairs[0][0].is_cuda:
-      return None, set()
-    fused = self._FusedModule(True)
+    fused = self._FusedModule(var_grad_pairs[0][0]) if var_grad_pairs else None
     if fused is None:
       return None, set()
     total = torch.zeros(1, dtype=torch.float32, device=var_grad_pairs[0][0].device)
@@ -781,7 +775,7 @@ class XLAShardingAdafactor(Base):
   def _Update(self, lr, variables, grads):
     p = self.params
     decay = self.DecayRate()
-    fused = self._FusedModule(variables[0].is_cuda)
+    fused = self._FusedModule(variables[0])
     hyper = getattr(self, '_hyper', None)
     pre = getattr(self, '_pre', {})
     self._pre = {}

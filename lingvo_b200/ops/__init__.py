@@ -8,7 +8,6 @@ PyTorch there. On CPU-only hosts the pure-PyTorch reference implementations
 """
 
 import importlib
-import os
 import threading
 
 import torch
@@ -57,15 +56,9 @@ def host():
   return _HOST
 
 
-def has_native() -> bool:
-  return native(required=False) is not None
-
-
 def use_cuda_kernels(*tensors) -> bool:
   """True when the fused sm_90a path must be taken for these tensors."""
   if not tensors or not all(t.is_cuda for t in tensors if t is not None):
-    return False
-  if os.environ.get('LINGVO_B200_DISABLE_KERNELS', '0') == '1':
     return False
   native(required=True)  # fail loudly on a GPU box without the extension
   return True

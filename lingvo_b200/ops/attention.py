@@ -129,9 +129,7 @@ class _FlashAttnFn(torch.autograd.Function):
 
 def flash_attention_supported(q, k, dropout_prob=0.0):
   from lingvo_b200 import ops
-  mod = ops.native(required=False) if q.is_cuda else None
-  return (mod is not None and hasattr(mod, '_has_flash_attn') and
-          ops.use_cuda_kernels(q) and q.dtype == torch.bfloat16 and q.dim() == 4 and
+  return (ops.use_cuda_kernels(q) and q.dtype == torch.bfloat16 and q.dim() == 4 and
           q.shape[-1] == 128 and q.shape[1] % 128 == 0 and k.dim() == 4 and
           k.shape[:2] == q.shape[:2] and k.shape[3] == 128 and k.shape[2] >= 1 and
           q.shape[2] % k.shape[2] == 0 and not dropout_prob)
@@ -194,9 +192,7 @@ def decode_attention_ref(q, k_new, v_new, k_cache, v_cache, t, rel=None, scale=1
 
 def decode_attention_supported(q, k_cache):
   from lingvo_b200 import ops
-  mod = ops.native(required=False) if q.is_cuda else None
-  return (mod is not None and hasattr(mod, '_has_decode_attn') and
-          ops.use_cuda_kernels(q, k_cache) and q.dtype == torch.bfloat16 and
+  return (ops.use_cuda_kernels(q, k_cache) and q.dtype == torch.bfloat16 and
           k_cache.dtype == torch.bfloat16 and q.dim() == 4 and k_cache.dim() == 4 and
           q.shape[-1] == 128 and k_cache.shape[-1] == 128 and
           q.shape[2] % k_cache.shape[2] == 0 and k_cache.is_contiguous())
@@ -286,9 +282,7 @@ def flat_beam_attention_ref(q, k_new, v_new, k_cache, v_cache, slot0, vis, qpos,
 
 def flat_beam_attention_supported(q, k_cache):
   from lingvo_b200 import ops
-  mod = ops.native(required=False) if q.is_cuda else None
-  return (mod is not None and hasattr(mod, '_has_flat_beam_attn') and
-          ops.use_cuda_kernels(q, k_cache) and q.dtype == torch.bfloat16 and
+  return (ops.use_cuda_kernels(q, k_cache) and q.dtype == torch.bfloat16 and
           k_cache.dtype == torch.bfloat16 and q.dim() == 4 and k_cache.dim() == 4 and
           1 <= q.shape[1] <= 16 and q.shape[-1] == 128 and k_cache.shape[-1] == 128 and
           q.shape[2] % k_cache.shape[2] == 0 and k_cache.is_contiguous())

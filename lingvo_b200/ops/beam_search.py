@@ -82,11 +82,10 @@ def _TopKRef(log_probs, cum, active, k, eos_id):
 
 def _TopK(log_probs, cum, active, k, eos_id):
   """Fused score-add + EOS mask + per-hyp top-K (`csrc/beam_kernels.cu` on the GPU)."""
-  if log_probs.is_cuda and k <= 16 and log_probs.dtype in (torch.float32, torch.bfloat16):
-    from lingvo_b200 import ops  # pylint: disable=g-import-not-at-top
-    nat = ops.native(required=False)
-    if nat is not None and hasattr(nat, '_has_beam'):
-      return tuple(nat.beam_topk(log_probs.contiguous(), cum, active, int(k), int(eos_id)))
+  from lingvo_b200 import ops  # pylint: disable=g-import-not-at-top
+  if (ops.use_cuda_kernels(log_probs) and k <= 16 and
+      log_probs.dtype in (torch.float32, torch.bfloat16)):
+    return tuple(ops.native().beam_topk(log_probs.contiguous(), cum, active, int(k), int(eos_id)))
   return _TopKRef(log_probs, cum, active, k, eos_id)
 
 

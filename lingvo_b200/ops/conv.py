@@ -40,9 +40,6 @@ def glu_dwconv1d_supported(x, conv_layer):
   """True when the fused kernel serves this depthwise conv layer. Kernel sizes above the
   backward's shared-memory limit (`glu_dwconv_max_k`) take the unfused path."""
   p = conv_layer.params
-  import os  # pylint: disable=g-import-not-at-top
-  if os.environ.get('LINGVO_B200_DISABLE_FUSED_CONV') == '1':   # A/B switch for benchmarks
-    return False
   return (ops.use_cuda_kernels(x) and x.dtype in (torch.bfloat16, torch.float32) and
           type(conv_layer).__name__ in ('DepthwiseConv2DLayer',
                                         'CausalDepthwiseConv2DLayer') and

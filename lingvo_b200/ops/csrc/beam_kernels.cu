@@ -169,6 +169,5 @@ std::vector<torch::Tensor> beam_topk(const torch::Tensor& log_probs, const torch
 }  // namespace lb
 
 LB_REGISTER(beam) {
-  m.attr("_has_beam") = true;
   m.def("beam_topk", &lb::beam_topk);
 }

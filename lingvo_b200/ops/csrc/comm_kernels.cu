@@ -255,7 +255,6 @@ void zero_adam(const torch::Tensor& grad_peers_cpu, const torch::Tensor& param_p
 }  // namespace lb
 
 LB_REGISTER(comm) {
-  m.attr("_has_comm") = true;
   m.def("allreduce_mean_bf16", &lb::allreduce_mean_bf16, pybind11::arg("peer_ptrs_cpu"),
         pybind11::arg("shard_elems"), pybind11::arg("rank"), pybind11::arg("world"),
         pybind11::arg("scale"), pybind11::arg("device"), pybind11::arg("store_all"),

@@ -277,7 +277,6 @@ std::vector<torch::Tensor> glu_dwconv1d_bwd(const torch::Tensor& proj, const tor
 }  // namespace lb
 
 LB_REGISTER(conv) {
-  m.attr("_has_conv") = true;
   m.attr("glu_dwconv_max_k") = lb::kMaxK;
   m.def("glu_dwconv1d_fwd", &lb::glu_dwconv1d_fwd);
   m.def("glu_dwconv1d_bwd", &lb::glu_dwconv1d_bwd);

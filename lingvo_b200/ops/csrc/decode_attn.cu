@@ -843,12 +843,10 @@ torch::Tensor flat_beam_attn_fwd(const torch::Tensor& q, const torch::Tensor& k_
 }  // namespace lb
 
 LB_REGISTER(decode_attn) {
-  m.attr("_has_decode_attn") = true;
   m.def("decode_attn_fwd", &lb::decode_attn_fwd, py::arg("q"), py::arg("k_new"), py::arg("v_new"),
         py::arg("k_cache"), py::arg("v_cache"), py::arg("t"), py::arg("rel"), py::arg("scale"));
   m.def("decode_attn_chunk", &lb::decode_attn_chunk, py::arg("B"), py::arg("H"), py::arg("Hk"),
         py::arg("T"));
-  m.attr("_has_flat_beam_attn") = true;
   m.def("flat_beam_attn_fwd", &lb::flat_beam_attn_fwd, py::arg("q"), py::arg("k_new"),
         py::arg("v_new"), py::arg("k_cache"), py::arg("v_cache"), py::arg("slot0"), py::arg("vis"),
         py::arg("qpos"), py::arg("kpos"), py::arg("rel"), py::arg("scale"));

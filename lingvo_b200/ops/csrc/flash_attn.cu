@@ -1034,7 +1034,6 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
 }  // namespace lb
 
 LB_REGISTER(flash_attn) {
-  m.attr("_has_flash_attn") = true;
   m.def("flash_attn_fwd", &lb::flash_attn_fwd, py::arg("q"), py::arg("k"), py::arg("v"),
         py::arg("rel"), py::arg("seg"), py::arg("pos"), py::arg("scale"), py::arg("causal"));
   m.def("flash_attn_bwd", &lb::flash_attn_bwd, py::arg("q"), py::arg("k"), py::arg("v"),

@@ -381,7 +381,6 @@ std::vector<torch::Tensor> gate_logits_bwd(const torch::Tensor& x, const torch::
 }  // namespace lb
 
 LB_REGISTER(gate) {
-  m.attr("_has_gate") = true;
   m.def("gate_logits_fwd", &lb::gate_logits_fwd);
   m.def("gate_logits_bwd", &lb::gate_logits_bwd);
 }

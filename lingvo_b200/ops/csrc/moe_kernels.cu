@@ -583,7 +583,6 @@ int64_t symm_import(const std::string& handle, int64_t device) {
 }  // namespace lb
 
 LB_REGISTER(moe) {
-  m.attr("_has_moe") = true;
   m.def("moe_gate_dispatch", &lb::moe_gate_dispatch);
   m.def("moe_scatter_rows", &lb::moe_scatter_rows);
   m.def("moe_combine", &lb::moe_combine);

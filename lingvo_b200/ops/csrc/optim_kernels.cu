@@ -808,7 +808,6 @@ void adam_flat(torch::Tensor w, const torch::Tensor& g, torch::Tensor m, torch::
 }  // namespace lb
 
 LB_REGISTER(optim) {
-  m.attr("_has_optim") = true;
   m.def("adafactor_stats", &lb::adafactor_stats);
   m.def("adafactor_update", &lb::adafactor_update);
   m.def("adafactor_small", &lb::adafactor_small);

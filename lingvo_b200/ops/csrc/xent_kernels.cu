@@ -187,7 +187,6 @@ void xent_bwd(torch::Tensor logits, const torch::Tensor& labels, const torch::Te
 }  // namespace lb
 
 LB_REGISTER(xent) {
-  m.attr("_has_xent") = true;
   m.def("xent_stats", &lb::xent_stats);
   m.def("xent_bwd", &lb::xent_bwd);
 }

@@ -11,15 +11,10 @@ from lingvo_b200 import ops
 _SUPPORTED_E = (2, 4, 8, 16)
 
 
-def available() -> bool:
-  mod = ops.native(required=False)
-  return mod is not None and hasattr(mod, '_has_gate')
-
-
 def supported(x, gw) -> bool:
   """The kernels read x with 16-byte loads, so a contiguous x must start 16-byte aligned (a
   strided x is copied first)."""
-  return (available() and x.is_cuda and x.dtype == torch.bfloat16 and gw.is_cuda and
+  return (ops.use_cuda_kernels(x, gw) and x.dtype == torch.bfloat16 and
           gw.device == x.device and (x.data_ptr() % 16 == 0 or not x.is_contiguous()) and
           gw.dtype in (torch.float32, torch.bfloat16) and gw.dim() == 2 and
           gw.shape[1] in _SUPPORTED_E and x.shape[-1] == gw.shape[0] and

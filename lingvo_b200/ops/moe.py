@@ -24,11 +24,6 @@ import torch
 from lingvo_b200 import ops
 
 
-def available() -> bool:
-  mod = ops.native(required=False)
-  return mod is not None and hasattr(mod, '_has_moe')
-
-
 def _Slots(index, pos, s, g_l, c):
   """Flat slot id `[2, T]` of each (choice, token) in an `[E, G_l, C]` buffer."""
   t = index.shape[-1]

@@ -5,18 +5,13 @@ import torch
 from lingvo_b200 import ops
 
 
-def available() -> bool:
-  mod = ops.native(required=False)
-  return mod is not None and hasattr(mod, '_has_norm')
-
-
 class _NormFn(torch.autograd.Function):
 
   @staticmethod
   def forward(ctx, x, scale, bias, eps, center):
     shape = x.shape
     x2 = x.contiguous().reshape(-1, shape[-1])
-    y, stats, _ = ops.native().norm_fwd(x2, None, scale, bias, eps, center, False)
+    y, stats = ops.native().norm_fwd(x2, scale, bias, eps, center)
     ctx.save_for_backward(x2, scale if scale is not None else torch.empty(0),
                           stats)
     ctx.center = center
@@ -55,7 +50,7 @@ class _NormPassFn(torch.autograd.Function):
   def forward(ctx, x, scale, eps):
     shape = x.shape
     x2 = x.contiguous().reshape(-1, shape[-1])
-    y, stats, _ = ops.native().norm_fwd(x2, None, scale, None, eps, False, False)
+    y, stats = ops.native().norm_fwd(x2, scale, None, eps, False)
     ctx.save_for_backward(x2, scale if scale is not None else torch.empty(0), stats)
     ctx.has_scale = scale is not None
     ctx.scale_dtype = scale.dtype if scale is not None else None

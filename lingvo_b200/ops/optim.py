@@ -9,11 +9,6 @@ from lingvo_b200 import ops
 _SCRATCH = {}
 
 
-def available() -> bool:
-  mod = ops.native(required=False)
-  return mod is not None and hasattr(mod, '_has_optim')
-
-
 def _Scratch(var, n):
   """Per-variable fp32 scratch; returns (buffer, fresh). `fresh` means the
   carried sum(w²) in it is not valid yet (first step, or after `Invalidate`)."""

@@ -14,11 +14,6 @@ from lingvo_b200.core.nested_map import NestedMap
 from lingvo_b200.ops import gemm
 
 
-def available() -> bool:
-  mod = ops.native(required=False)
-  return mod is not None and hasattr(mod, '_has_xent')
-
-
 class _LmHeadXent(torch.autograd.Function):
 
   @staticmethod

@@ -15,7 +15,6 @@ Two engines, both built on `comm_kernels.cu` + the flag protocol:
 from __future__ import annotations
 
 import math
-import os
 from typing import List
 
 import torch
@@ -87,7 +86,7 @@ class FusedAllReduce:
   _COMM_BLOCKS = 48
   _MAX_BUCKETS = 60
 
-  def __init__(self, task, ctx, overlap: bool = True, bucket_bytes: int = 48 << 20):
+  def __init__(self, task, ctx, bucket_bytes: int = 48 << 20):
     self.ctx = ctx
     self.world, self.rank = ctx.world, ctx.rank
     dev = task.Device()
@@ -101,8 +100,7 @@ class FusedAllReduce:
                               dtype=torch.int64)
     self.chan = _Channels(self.arena, self.world, self.rank, n=2 * self._MAX_BUCKETS + 8)
     self._index = {id(v): i for i, v in enumerate(self.flat.vars)}
-    self._overlap = (bool(overlap) and dev.type == 'cuda' and
-                     os.environ.get('LINGVO_B200_DP_OVERLAP', '1') != '0')
+    self._overlap = dev.type == 'cuda'
     self._bucket_bytes = int(bucket_bytes)
     self._arrival: List[int] = []
     self._phase = 0                      # 0: learning the order, 1: overlapped

@@ -159,7 +159,7 @@ def _Inputs(rows, dim, seed, offset=0.0):
 def _CheckNative(x, dy, scale, bias, center, need_ds=True, need_db=True, what=''):
   """norm_fwd + norm_bwd through the bindings against the oracle; returns the outputs."""
   nat = ops.native()
-  y, stats, _ = nat.norm_fwd(x, None, scale, bias, _EPS, center, False)
+  y, stats = nat.norm_fwd(x, scale, bias, _EPS, center)
   o = _Oracle(x, dy, scale, bias, center)
   assert stats.shape == (x.shape[0], 2) and stats.dtype == torch.float32
   # where a bias cancels x̂·scale, the rstd's own error (bounded below) may exceed an ulp of y
@@ -205,7 +205,7 @@ def test_rms_norm_benchmark_shape(scale_dtype):
   _AssertBf16(y.detach(), o['y'], o['slack_y'] + _Ulp(o['y']), 'y')
   _AssertBf16(xg.grad, o['dx'], o['slack_dx'] + _Ulp(o['dx']), 'dx')
   # the fp32 dscale the kernels fold, and its single rounding to the parameter's dtype
-  _, stats, _ = ops.native().norm_fwd(x, None, scale, None, _EPS, False, False)
+  _, stats = ops.native().norm_fwd(x, scale, None, _EPS, False)
   assert bool((stats[:, 0] == 0).all())
   _AssertWithin(stats[:, 1], o['rstd'], o['d_rstd'], 'rstd')
   assert float((o['d_rstd'] / o['rstd']).max()) <= 2 * 2.0**-16
@@ -256,7 +256,7 @@ def test_backward_is_bitwise_reproducible(center):
   x, dy, scale, bias = _Inputs(rows, dim, 4)
   dres = _Inputs(rows, dim, 5)[1]
   nat = ops.native()
-  _, stats, _ = nat.norm_fwd(x, None, scale, bias if center else None, _EPS, center, False)
+  _, stats = nat.norm_fwd(x, scale, bias if center else None, _EPS, center)
   runs = [nat.norm_bwd(x, dy, dres, scale, stats, center, True, center) for _ in range(3)]
   for dx, ds, db in runs[1:]:
     assert torch.equal(dx, runs[0][0]) and torch.equal(ds, runs[0][1])
@@ -418,28 +418,25 @@ def test_norm_fwd_refusals():
   nat = ops.native()
   x = torch.randn(16, 64, device='cuda').bfloat16()
   s = torch.ones(64, device='cuda')
-  _Refused(lambda: nat.norm_fwd(x.float(), None, s, None, _EPS, True, False), 'bf16')
-  _Refused(lambda: nat.norm_fwd(x[:, :60].contiguous(), None, None, None, _EPS, True, False),
+  _Refused(lambda: nat.norm_fwd(x.float(), s, None, _EPS, True), 'bf16')
+  _Refused(lambda: nat.norm_fwd(x[:, :60].contiguous(), None, None, _EPS, True),
            'multiple of 8')
-  _Refused(lambda: nat.norm_fwd(x, None, s[:56], None, _EPS, True, False), 'scale')
-  _Refused(lambda: nat.norm_fwd(x, None, s, torch.ones(72, device='cuda'), _EPS, True, False),
-           'bias')
-  _Refused(lambda: nat.norm_fwd(x, x[:8], None, None, _EPS, False, False), 'res')
+  _Refused(lambda: nat.norm_fwd(x, s[:56], None, _EPS, True), 'scale')
+  _Refused(lambda: nat.norm_fwd(x, s, torch.ones(72, device='cuda'), _EPS, True), 'bias')
   # a contiguous bf16 view at a storage offset of 4 elements (8 bytes)
   flat = torch.randn(16 * 64 + 8, device='cuda').bfloat16()
   xv = flat[4:4 + 16 * 64].view(16, 64)
   assert xv.is_contiguous() and xv.data_ptr() % 16 == 8
-  _Refused(lambda: nat.norm_fwd(xv, None, s, None, _EPS, True, False), 'aligned')
-  _Refused(lambda: nat.norm_fwd(x, xv, s, None, _EPS, True, False), 'res')
+  _Refused(lambda: nat.norm_fwd(xv, s, None, _EPS, True), 'aligned')
   sflat = torch.ones(72, device='cuda')
-  _Refused(lambda: nat.norm_fwd(x, None, sflat[2:66], None, _EPS, True, False), 'aligned')
+  _Refused(lambda: nat.norm_fwd(x, sflat[2:66], None, _EPS, True), 'aligned')
 
 
 def test_norm_bwd_refusals():
   nat = ops.native()
   x = torch.randn(16, 64, device='cuda').bfloat16()
   s = torch.ones(64, device='cuda')
-  _, stats, _ = nat.norm_fwd(x, None, s, None, _EPS, False, False)
+  _, stats = nat.norm_fwd(x, s, None, _EPS, False)
   dy = torch.randn_like(x)
   flat = torch.randn(16 * 64 + 8, device='cuda').bfloat16()
   xv = flat[4:4 + 16 * 64].view(16, 64)

@@ -18,7 +18,6 @@ import torch
 
 
 def Run(model_name, streams, graph, steps):
-  os.environ['LINGVO_B200_ADAFACTOR_STREAMS'] = str(streams)
   from lingvo_b200 import model_registry
   from lingvo_b200.core import cluster_factory, py_utils
   from lingvo_b200.ops import optim
@@ -33,6 +32,7 @@ def Run(model_name, streams, graph, steps):
   cfg = model_registry.GetParams(model_name, 'Train')
   cfg.task.random_seed = 1
   cfg.input.random_seed = 5
+  cfg.task.train.optimizer.num_update_streams = streams
   cfg.cluster.worker.gpus_per_replica = 1
   dev = torch.device('cuda', 0)
   with cluster_factory.Cluster(cfg.cluster):

@@ -5,6 +5,7 @@ Writes gpurun_out/conformer_bench.json."""
 import json
 import os
 import sys
+from unittest import mock
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -72,11 +73,9 @@ def main():
     torch.autograd.grad(y.float().sum(), [h] + [v for v in lc.vars.Flatten() if v.requires_grad],
                         allow_unused=True)
   out['lconv_fused_ms'] = Time(lconv)
-  os.environ['LINGVO_B200_DISABLE_FUSED_CONV'] = '1'
-  try:
+  from lingvo_b200.ops import conv as conv_ops
+  with mock.patch.object(conv_ops, 'glu_dwconv1d_supported', lambda *a: False):
     out['lconv_unfused_ms'] = Time(lconv)
-  finally:
-    del os.environ['LINGVO_B200_DISABLE_FUSED_CONV']
   os.makedirs('gpurun_out', exist_ok=True)
   json.dump(out, open('gpurun_out/conformer_bench.json', 'w'), indent=1)
   print(json.dumps(out))
