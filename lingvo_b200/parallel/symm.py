@@ -106,6 +106,8 @@ class _LayerBufs:
     self._ex, self._geom = ex, (g_l, c, m)
     self.chan = ex.NewChannels(4)
     self.seq = [0, 0, 0, 0]
+    # Bumped by every forward that refills xe / yc, which hold its data until backward.
+    self.generation = 0
 
   @property
   def peer_xe(self):
@@ -252,6 +254,7 @@ class MoeExchange:
     """x2d `[G_l·S, M]`, logits `[G_l, S, E]` → (y `[G_l·S, M]`, aux_loss)."""
     g_l, s, e = logits.shape
     bufs, g = self.GateAndDispatch(key, x2d, logits, paddings, capacity, legacy)
+    bufs.generation += 1
     # Differentiable gate values (tiny [G,S,E] tensors) for the chosen experts.
     raw = torch.softmax(logits.float(), dim=-1)
     nonpad = None if paddings is None else (1.0 - paddings.float())
@@ -300,16 +303,23 @@ class _MoeFn(torch.autograd.Function):
     pos = g.pos.reshape(2, -1).contiguous()
     y = nat.moe_combine(bufs.yc, g.index, g.pos, gate_v.view(2, g_l, s), s, g_l,
                         c)
-    ctx.save_for_backward(gate_v, wi, wo, h)
+    # xe / yc stay in the layer's symmetric buffers until backward. The generation that
+    # filled them is a saved tensor, not a ctx attribute: a rematerialised forward re-runs
+    # `Apply` and refreshes the saved tensors of the original node.
+    ctx.save_for_backward(gate_v, wi, wo, h, torch.tensor(bufs.generation))
     ctx.ex, ctx.bufs, ctx.g, ctx.dims = ex, bufs, g, (g_l, s, c)
-    # xe / yc stay in the layer's symmetric buffers until backward.
     return y
 
   @staticmethod
   def backward(ctx, dy):
     nat = ops.native()
-    gate_v, wi, wo, h = ctx.saved_tensors
+    gate_v, wi, wo, h, generation = ctx.saved_tensors
     ex, bufs, g = ctx.ex, ctx.bufs, ctx.g
+    if int(generation) != bufs.generation:
+      raise RuntimeError(
+          'MoeExchange: this MoE layer ran forward again before the backward of an earlier '
+          'forward; its expert buffers now hold the later forward\'s data. Run each forward\'s '
+          'backward before the next forward of the same layer, or rematerialise it.')
     g_l, s, c = ctx.dims
     dy = dy.contiguous()
     gate3 = gate_v.view(2, g_l, s)

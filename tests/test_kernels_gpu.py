@@ -153,49 +153,6 @@ def test_ffn_relu():
     assert _rel(a, b) < 3e-2
 
 
-@pytest.mark.parametrize('legacy,g,s,m,h', [
-    pytest.param(True, 4, 128, 256, 512, id='True'),
-    pytest.param(False, 4, 128, 256, 512, id='False'),
-    # S = 1024: the gate's position scan carries counts across 4 chunks of 256 tokens.
-    pytest.param(True, 2, 1024, 512, 1024, id='s1024-True'),
-    pytest.param(False, 2, 1024, 512, 1024, id='s1024-False'),
-])
-def test_moe_exchange_matches_dense_oracle(legacy, g, s, m, h):
-  """Fused gate+dispatch / expert GEMMs / combine == dense GSEC einsums."""
-  from lingvo_b200.core import gshard_layers
-  from lingvo_b200.parallel import symm
-  torch.manual_seed(1)
-  e = 8
-  cap = gshard_layers.ExpertCapacity(s, e, 0, 2.0)
-  x = torch.randn(g, s, m, device='cuda').bfloat16().requires_grad_()
-  gw = (torch.randn(m, e, device='cuda') * 0.2).requires_grad_()
-  wi = (torch.randn(e, m, h, device='cuda') * 0.05).bfloat16().requires_grad_()
-  wo = (torch.randn(e, h, m, device='cuda') * 0.05).bfloat16().requires_grad_()
-  pad = torch.zeros(g, s, device='cuda')
-  pad[:, -7:] = 1.0
-  ex = symm.MoeExchange(None, e, torch.device('cuda', 0))
-  logits = torch.matmul(x.float(), gw)
-  y, aux = ex.Apply(('t', legacy), x.reshape(g * s, m), logits, pad, cap, legacy,
-                    wi, wo)
-  dy = torch.randn_like(y)
-  (y.float() * dy.float()).sum().add(aux * 3.0).backward()
-
-  xr, gwr, wir, wor = [t.detach().float().requires_grad_()
-                       for t in (x, gw, wi, wo)]
-  gating = gshard_layers.ComputeGating(
-      gwr, xr, pad, 1, e, 0, True, torch.float32, 'top_2', False, 'all', 0.0,
-      legacy, 2.0, None, torch.float32, torch.float32)
-  yr, auxr = gshard_layers.FeedForwardNetworksApplyGating(
-      gating, xr, xr, wir, wor, 1, g)
-  (yr.reshape(g * s, m) * dy.float()).sum().add(auxr * 3.0).backward()
-  assert _rel(y, yr.reshape(g * s, m)) < 3e-2
-  assert abs(float(aux) - float(auxr)) < 1e-4
-  assert _rel(x.grad, xr.grad) < 5e-2
-  assert _rel(gw.grad, gwr.grad) < 5e-2
-  assert _rel(wi.grad, wir.grad) < 5e-2
-  assert _rel(wo.grad, wor.grad) < 5e-2
-
-
 @pytest.mark.parametrize('causal', [False, True])
 @pytest.mark.parametrize('dtype', [torch.bfloat16, torch.float32])
 def test_glu_dwconv1d_kernel(causal, dtype):
