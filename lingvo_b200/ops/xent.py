@@ -47,6 +47,9 @@ class _LmHeadXent(torch.autograd.Function):
     c = d_soft * (on - off) + d_ent
     ops.native().xent_bwd(logits, labels, lse, a.contiguous(), b.contiguous(),
                           c.contiguous())
+    # The saved logits now hold dlogits: a second backward through a retained graph must
+    # raise autograd's in-place-modification error instead of reading them as logits.
+    torch.autograd.graph.increment_version(logits)
     dlogits = logits                                       # rewritten in place
     dx = dw = None
     if ctx.needs_input_grad[0]:
