@@ -4,8 +4,10 @@ Reference `lingvo/core/gshard_layers.py`:
   * `Top2GatingOnLogits` (:1932-2364) — reproduced verbatim in *math* as the
     dense `GSEC` oracle (`Top2GatingOnLogits`), and re-designed as an
     **index-based** gate (`Top2GatingIndices`) that returns
-    `(expert, slot, gate) × 2` per token — what the fused sm_90a gate kernel
-    (`ops.moe.top2_gate`) produces. Both implement: softmax over E, top-1,
+    `(expert, slot, gate) × 2` per token — the routing the fused sm_90a gate +
+    dispatch kernel (`moe_gate_dispatch`, run by `parallel.symm.MoeExchange`)
+    produces. `Top2Gates` computes the differentiable gate values and aux loss
+    of a given routing for both. Both implement: softmax over E, top-1,
     second-expert policy (`all` / `sampling` (Gumbel) / `random` threshold),
     exclusive cumsum positions with first-choice priority (:2230, :2294),
     capacity rounding ↑4 (:2062-2076), renorm before/after capacity
@@ -191,6 +193,60 @@ def Top2GatingOnLogits(inputs, paddings, logits, num_devices, experts_dim,
   return aux_loss, combine_tensor, dispatch_tensor
 
 
+def _Top2GatesBeforeCapacity(logits, paddings, index, legacy_mtf_behavior):
+  """→ (gate_1, gate_2, aux_loss) of the chosen experts `index`, before capacity.
+
+  As if read from the softmax with the top-1 entry removed, `gate_2` is 0 where
+  the second choice repeats the first (padding, or underflow to 0)."""
+  e = logits.shape[-1]
+  raw = torch.softmax(logits.float(), dim=-1)
+  nonpad = None if paddings is None else (1.0 - paddings.float())
+  index_1, index_2 = index[0].long(), index[1].long()
+  oh1 = F.one_hot(index_1, e).float()
+  gate_1 = torch.gather(raw, -1, index_1.unsqueeze(-1)).squeeze(-1)
+  gate_2 = torch.gather(raw, -1, index_2.unsqueeze(-1)).squeeze(-1)
+  live_2 = index_2 != index_1
+  proxy = raw
+  if nonpad is not None:
+    oh1 = oh1 * nonpad.unsqueeze(-1)
+    proxy = raw * nonpad.unsqueeze(-1)
+    gate_1 = gate_1 * nonpad
+    live_2 = live_2 & (nonpad > 0)
+  gate_2 = gate_2 * live_2
+  if legacy_mtf_behavior:
+    denom = gate_1 + gate_2 + 1e-9
+    gate_1, gate_2 = gate_1 / denom, gate_2 / denom
+  density_denom = 1.0 if legacy_mtf_behavior else (
+      (nonpad if nonpad is not None else torch.ones_like(gate_1)).mean(1)[:, None]
+      + 1e-6)
+  density_1 = oh1.mean(dim=1) / density_denom
+  aux_loss = ((proxy.mean(dim=1) / density_denom) * density_1).mean() * (e * e)
+  return gate_1, gate_2, aux_loss
+
+
+def _Top2GatesAfterCapacity(gate_1, gate_2, keep, legacy_mtf_behavior):
+  """Zeroes the gates of dropped choices; without `legacy_mtf_behavior` the kept
+  pair is then renormalised to sum to 1. → gate `[2, G, S]`."""
+  gate_1 = gate_1 * keep[0].float()
+  gate_2 = gate_2 * keep[1].float()
+  if not legacy_mtf_behavior:
+    denom = gate_1 + gate_2
+    denom = torch.where(denom > 0, denom, torch.ones_like(denom))
+    gate_1, gate_2 = gate_1 / denom, gate_2 / denom
+  return torch.stack([gate_1, gate_2])
+
+
+def Top2Gates(logits, paddings, index, keep, legacy_mtf_behavior):
+  """Top-2 gate values and aux loss of a routing, differentiable w.r.t. logits.
+
+  index `[2, G, S]` holds the chosen experts, keep `[2, G, S]` is true (or 1)
+  where the choice was dispatched. → (gate `[2, G, S]` fp32, aux_loss)."""
+  gate_1, gate_2, aux_loss = _Top2GatesBeforeCapacity(logits, paddings, index,
+                                                      legacy_mtf_behavior)
+  return (_Top2GatesAfterCapacity(gate_1, gate_2, keep, legacy_mtf_behavior),
+          aux_loss)
+
+
 def Top2GatingIndices(logits, paddings, experts_dim, expert_capacity_dim,
                       fprop_dtype=torch.float32, second_expert_policy='all',
                       second_expert_threshold=0.0, legacy_mtf_behavior=True,
@@ -212,39 +268,27 @@ def Top2GatingIndices(logits, paddings, experts_dim, expert_capacity_dim,
   nonpad = None if paddings is None else (1.0 - paddings.float())
   index_1 = raw.argmax(-1)
   oh1 = F.one_hot(index_1, e).float()
-  proxy = raw
   if nonpad is not None:
     oh1 = oh1 * nonpad.unsqueeze(-1)
-    proxy = raw * nonpad.unsqueeze(-1)
-  gate_1 = torch.gather(raw, -1, index_1.unsqueeze(-1)).squeeze(-1)
-  if nonpad is not None:
-    gate_1 = gate_1 * nonpad
-  wo1 = raw.scatter(-1, index_1.unsqueeze(-1), 0.0) if nonpad is None else (
-      raw * (1.0 - oh1))
   if second_expert_policy == 'sampling':
     noise = _Gumbel(logits.shape, logits.device, torch.float32, seeds)
     very_neg = torch.finfo(torch.float32).max * -0.7
     upd = torch.where(oh1 > 0, torch.full_like(raw, very_neg), logits.float())
     index_2 = (upd + noise).argmax(-1)
   else:
-    index_2 = wo1.argmax(-1)
+    # A padded token keeps its top-1 entry, so its second choice repeats it.
+    index_2 = (raw * (1.0 - oh1)).argmax(-1)
   oh2 = F.one_hot(index_2, e).float()
   if nonpad is not None:
     oh2 = oh2 * (nonpad > 0).float().unsqueeze(-1)
-  gate_2 = (wo1 * oh2).sum(-1)
-  if legacy_mtf_behavior:
-    denom = gate_1 + gate_2 + 1e-9
-    gate_1, gate_2 = gate_1 / denom, gate_2 / denom
+  index = torch.stack([index_1, index_2])
+  # `random` samples on gate_2 after the legacy renormalisation, before capacity.
+  gate_1, gate_2, aux_loss = _Top2GatesBeforeCapacity(logits, paddings, index,
+                                                      legacy_mtf_behavior)
   pos1_all = torch.cumsum(oh1, dim=1) - oh1
-  density_denom = 1.0 if legacy_mtf_behavior else (
-      (nonpad if nonpad is not None else torch.ones_like(gate_1)).mean(1)[:, None]
-      + 1e-6)
-  density_1 = oh1.mean(dim=1) / density_denom
-  aux_loss = ((proxy.mean(dim=1) / density_denom) * density_1).mean() * (e * e)
   keep1 = oh1 * (pos1_all < cap).float()
   pos1 = (pos1_all * keep1).sum(-1)
   count1 = keep1.sum(dim=1)
-  flat1 = keep1.sum(-1)
   if second_expert_policy == 'random':
     gen = None
     if seeds is not None:
@@ -252,18 +296,13 @@ def Top2GatingIndices(logits, paddings, experts_dim, expert_capacity_dim,
       gen.manual_seed(((int(seeds[0]) & 0x7fffffff) << 31) ^ int(seeds[1]) ^ 7)
     u = torch.rand(gate_2.shape, device=gate_2.device, generator=gen)
     sampled = (u < gate_2 / max(second_expert_threshold, 1e-9)).float()
-    gate_2 = gate_2 * sampled
     oh2 = oh2 * sampled.unsqueeze(-1)
   pos2_all = torch.cumsum(oh2, dim=1) - oh2 + count1.unsqueeze(1)
   keep2 = oh2 * (pos2_all < cap).float()
   pos2 = (pos2_all * keep2).sum(-1)
-  flat2 = keep2.sum(-1)
-  gate_1 = gate_1 * flat1
-  gate_2 = gate_2 * flat2
-  if not legacy_mtf_behavior:
-    denom = gate_1 + gate_2
-    denom = torch.where(denom > 0, denom, torch.ones_like(denom))
-    gate_1, gate_2 = gate_1 / denom, gate_2 / denom
+  gate = _Top2GatesAfterCapacity(gate_1, gate_2,
+                                 (keep1.sum(-1), keep2.sum(-1)),
+                                 legacy_mtf_behavior)
   with torch.no_grad():
     over1 = (oh1.sum() - keep1.sum())
     over2 = (oh2.sum() - keep2.sum())
@@ -271,9 +310,9 @@ def Top2GatingIndices(logits, paddings, experts_dim, expert_capacity_dim,
   summary_utils.scalar('over_capacity_1', over1)
   summary_utils.scalar('over_capacity_2', over2)
   return NestedMap(
-      index=torch.stack([index_1, index_2]).to(torch.int32),
+      index=index.to(torch.int32),
       pos=torch.stack([pos1, pos2]).to(torch.int32),
-      gate=torch.stack([gate_1, gate_2]), aux_loss=aux_loss, capacity=cap)
+      gate=gate, aux_loss=aux_loss, capacity=cap)
 
 
 def CombineTensorFromIndices(gating: NestedMap, experts_dim: int):
@@ -417,8 +456,9 @@ def FeedForwardNetworksApplyGating(gating, inputs, reshaped_inputs, wi_split,
 
 
 # --------------------------------------------------------------------------
-# Index-based dispatch / combine (single device). The expert-parallel variant
-# lives in lingvo_b200.parallel.ep and shares these slot conventions:
+# Index-based dispatch / combine. Under expert parallelism
+# lingvo_b200.parallel.ep moves the dispatched rows between ranks; both sides
+# use these slot conventions:
 #   slot(e, g, c) = (e * G + g) * C + c   in a [E, G*C, M] buffer.
 # --------------------------------------------------------------------------
 def _Slots(gating: NestedMap, g: int, s: int):
@@ -483,11 +523,10 @@ def MoEApplyIndexed(x, gating: NestedMap, wi, wo, activation_name='RELU',
   from lingvo_b200.ops import gemm
   g, s, m = x.shape
   e = wi.shape[-3] if ep_engine is None else ep_engine.num_experts
-  x2d = x.reshape(g * s, m)
+  xin = MoEDispatchIndexed(x.reshape(g * s, m), gating, g, s, e)
   if ep_engine is not None:
-    return ep_engine.Apply(x2d, gating, wi, wo, activation_name, bi, bo,
-                           use_glu).reshape(g, s, m)
-  xin = MoEDispatchIndexed(x2d, gating, g, s, e)
+    xin = ep_engine.ToExperts(xin)
+    wi, wo = ep_engine.ScaleExpertGrad(wi), ep_engine.ScaleExpertGrad(wo)
   if use_glu:
     h0 = gemm.grouped_linear(xin, wi[0].to(xin.dtype))
     h1 = gemm.grouped_linear(xin, wi[1].to(xin.dtype))
@@ -498,6 +537,8 @@ def MoEApplyIndexed(x, gating: NestedMap, wi, wo, activation_name='RELU',
     h = activations.GetFn(activation_name)(
         gemm.grouped_linear(xin, wi.to(xin.dtype), bi))
   out = gemm.grouped_linear(h, wo.to(h.dtype), bo)
+  if ep_engine is not None:
+    out = ep_engine.FromExperts(out)
   return MoECombineIndexed(out, gating, g, s).reshape(g, s, m)
 
 

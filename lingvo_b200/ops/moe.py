@@ -16,7 +16,8 @@ expert e.
 engine; their math oracle is `top2_gate_ref` below (`core/gshard_layers.Top2GatingIndices`),
 and `tests/test_moe_routing_gpu.py` checks both kernels against it: index, pos, gate and slot
 table exactly, and every expert-buffer row bitwise. The row movers below are plain tensor →
-tensor and are exposed here with `*_ref` oracles like every other op module.
+tensor; the exchange calls them through this module, and each has a `*_ref` oracle like every
+other op module.
 """
 
 import torch

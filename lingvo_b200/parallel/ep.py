@@ -5,7 +5,8 @@ XLA all-to-all (`gshard_layers.py:3072-3161`), TPU-only. Here it is explicit:
 
 * `mode='nccl'`  — stock baseline: local index-dispatch into `[E, G_l·C, M]`,
   `all_to_all_single`, grouped expert GEMMs, `all_to_all_single`, local
-  index-combine.
+  index-combine (`gshard_layers.MoEApplyIndexed`, with `ToExperts` /
+  `FromExperts` below as the two exchanges).
 * `mode='fused'` — the H100 path (`ops/moe.py` + `parallel/symm.py`): the
   dispatch kernel writes every routed token row **directly into the owning
   rank's expert buffer over NVLink** (peer stores into symmetric memory), the
@@ -22,10 +23,6 @@ from __future__ import annotations
 
 import torch
 import torch.distributed as dist
-
-from lingvo_b200.core import activations
-from lingvo_b200.core import gshard_layers
-from lingvo_b200.core.nested_map import NestedMap
 
 
 class _AllToAll(torch.autograd.Function):
@@ -81,7 +78,6 @@ class ExpertParallel:
           self.group = g
       self.ep_rank = ctx.rank % ep_size
     self._fused = None
-    self.last_a2a_ms = 0.0
 
   def GetExchange(self, device):
     """The fused peer-memory exchange, or None (NCCL baseline / CPU)."""
@@ -92,34 +88,23 @@ class ExpertParallel:
         self._fused = symm.MoeExchange(self, device=device)
     return self._fused or None
 
-  def Apply(self, x2d, gating: NestedMap, wi, wo, activation_name='RELU',
-            bi=None, bo=None, use_glu=False):
-    """tokens `[G_l·S, M]` → `[G_l·S, M]`; `wi/wo` hold the local experts."""
-    from lingvo_b200.ops import gemm
-    g_l = gating.index.shape[1]
-    s = gating.index.shape[2]
-    e, ep, el = self.num_experts, self.ep_size, self.num_local_experts
-    c = gating.capacity
-    m = x2d.shape[-1]
-    if ep > 1 and torch.is_grad_enabled():
-      wi = _ScaleGrad.apply(wi, 1.0 / ep)
-      wo = _ScaleGrad.apply(wo, 1.0 / ep)
-    xin = gshard_layers.MoEDispatchIndexed(x2d, gating, g_l, s, e)  # [E,Gl*C,M]
-    send = xin.reshape(ep, el * g_l * c, m)
-    recv = _AllToAll.apply(send, self.group)          # [src, El*Gl*C, M]
-    xe = recv.reshape(ep, el, g_l * c, m).transpose(0, 1).reshape(
-        el, ep * g_l * c, m)
-    if use_glu:
-      h = activations.GetFn(activation_name)(
-          gemm.grouped_linear(xe, wi[0].to(xe.dtype))) * gemm.grouped_linear(
-              xe, wi[1].to(xe.dtype))
-    elif activation_name in ('RELU', 'NONE'):
-      h = gemm.grouped_linear(xe, wi.to(xe.dtype), bi, act=activation_name)
-    else:
-      h = activations.GetFn(activation_name)(
-          gemm.grouped_linear(xe, wi.to(xe.dtype), bi))
-    ye = gemm.grouped_linear(h, wo.to(h.dtype), bo)   # [El, ep*Gl*C, M]
-    back = ye.reshape(el, ep, g_l * c, m).transpose(0, 1).reshape(
-        ep, el * g_l * c, m)
-    out = _AllToAll.apply(back, self.group).reshape(e, g_l * c, m)
-    return gshard_layers.MoECombineIndexed(out, gating, g_l, s)
+  def ScaleExpertGrad(self, w):
+    """Local expert weights whose gradient is scaled by 1/ep while training."""
+    if self.ep_size > 1 and torch.is_grad_enabled():
+      return _ScaleGrad.apply(w, 1.0 / self.ep_size)
+    return w
+
+  def ToExperts(self, xin):
+    """This rank's expert inputs `[E, G_l·C, M]` → the local experts' inputs
+    from every rank `[E_local, ep·G_l·C, M]`."""
+    _, rows, m = xin.shape
+    ep, el = self.ep_size, self.num_local_experts
+    recv = _AllToAll.apply(xin.reshape(ep, el * rows, m), self.group)
+    return recv.reshape(ep, el, rows, m).transpose(0, 1).reshape(el, ep * rows, m)
+
+  def FromExperts(self, ye):
+    """Inverse of `ToExperts`: `[E_local, ep·G_l·C, M]` → `[E, G_l·C, M]`."""
+    el, ep = self.num_local_experts, self.ep_size
+    rows, m = ye.shape[1] // ep, ye.shape[2]
+    back = ye.reshape(el, ep, rows, m).transpose(0, 1).reshape(ep, el * rows, m)
+    return _AllToAll.apply(back, self.group).reshape(self.num_experts, rows, m)

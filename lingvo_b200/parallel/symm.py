@@ -20,6 +20,9 @@ all ranks.
             GEMM with fused ReLU-mask epilogue, two wgrad GEMMs, dgrad GEMM
             with the row-pointer epilogue back to the sources, token gather.
 
+The routing is the kernel's; its differentiable gate values and aux loss come
+from `gshard_layers.Top2Gates`.
+
 With a single rank the very same kernels run on local pointers.
 """
 
@@ -30,11 +33,12 @@ from typing import Dict, Optional
 
 import torch
 import torch.distributed as dist
-import torch.nn.functional as F
 
 from lingvo_b200 import ops
+from lingvo_b200.core import gshard_layers
 from lingvo_b200.core.nested_map import NestedMap
 from lingvo_b200.ops import gemm
+from lingvo_b200.ops import moe
 
 _ALIGN = 1024
 
@@ -252,38 +256,11 @@ class MoeExchange:
 
   def Apply(self, key, x2d, logits, paddings, capacity, legacy, wi, wo):
     """x2d `[G_l·S, M]`, logits `[G_l, S, E]` → (y `[G_l·S, M]`, aux_loss)."""
-    g_l, s, e = logits.shape
+    g_l, s, _ = logits.shape
     bufs, g = self.GateAndDispatch(key, x2d, logits, paddings, capacity, legacy)
     bufs.generation += 1
-    # Differentiable gate values (tiny [G,S,E] tensors) for the chosen experts.
-    raw = torch.softmax(logits.float(), dim=-1)
-    nonpad = None if paddings is None else (1.0 - paddings.float())
-    i1, i2 = g.index[0].long(), g.index[1].long()
-    g1 = raw.gather(-1, i1.unsqueeze(-1)).squeeze(-1)
-    g2 = raw.gather(-1, i2.unsqueeze(-1)).squeeze(-1)
-    oh1 = F.one_hot(i1, e).float()
-    proxy = raw
-    if nonpad is not None:
-      g1, g2 = g1 * nonpad, g2 * nonpad
-      oh1 = oh1 * nonpad.unsqueeze(-1)
-      proxy = raw * nonpad.unsqueeze(-1)
-    if legacy:
-      den = g1 + g2 + 1e-9
-      g1, g2 = g1 / den, g2 / den
-    g1 = g1 * g.keep[0].float()
-    g2 = g2 * g.keep[1].float()
-    if not legacy:
-      den = g1 + g2
-      den = torch.where(den > 0, den, torch.ones_like(den))
-      g1, g2 = g1 / den, g2 / den
-    if legacy:
-      dden = 1.0
-    else:
-      imp = nonpad if nonpad is not None else torch.ones_like(g1)
-      dden = imp.mean(1)[:, None] + 1e-6
-    aux_loss = ((proxy.mean(1) / dden) * (oh1.mean(1) / dden)).mean() * (e * e)
-    gate = torch.stack([g1, g2]).reshape(2, g_l * s)
-    y = _MoeFn.apply(x2d, gate, wi, wo, self, bufs, g, g_l, s)
+    gate, aux_loss = gshard_layers.Top2Gates(logits, paddings, g.index, g.keep, legacy)
+    y = _MoeFn.apply(x2d, gate.reshape(2, g_l * s), wi, wo, self, bufs, g, g_l, s)
     return y, aux_loss
 
 
@@ -292,17 +269,13 @@ class _MoeFn(torch.autograd.Function):
   @staticmethod
   def forward(ctx, x2d, gate, wi, wo, ex: MoeExchange, bufs: _LayerBufs,
               g: NestedMap, g_l, s):
-    nat = ops.native()
     c = g.capacity
     ex._Sync(bufs, 0)                                   # dispatch rows landed
     h = gemm.gemm(bufs.xe, wi, True, False, act='RELU')  # [El, A, H]
     gemm.gemm(h, wo, True, False, row_ptrs=bufs.row_ptrs_yc)   # → peers' yc
     ex._Sync(bufs, 1)                                   # combine rows landed
     gate_v = gate.detach().float().contiguous()
-    idx = g.index.reshape(2, -1).contiguous()
-    pos = g.pos.reshape(2, -1).contiguous()
-    y = nat.moe_combine(bufs.yc, g.index, g.pos, gate_v.view(2, g_l, s), s, g_l,
-                        c)
+    y = moe.combine(bufs.yc, g.index, g.pos, gate_v, s, g_l, c)
     # xe / yc stay in the layer's symmetric buffers until backward. The generation that
     # filled them is a saved tensor, not a ctx attribute: a rematerialised forward re-runs
     # `Apply` and refreshes the saved tensors of the original node.
@@ -322,9 +295,7 @@ class _MoeFn(torch.autograd.Function):
           'backward before the next forward of the same layer, or rematerialise it.')
     g_l, s, c = ctx.dims
     dy = dy.contiguous()
-    gate3 = gate_v.view(2, g_l, s)
-    dgate = nat.moe_combine_bwd_gate(bufs.yc, dy, g.index, g.pos, gate3, s, g_l,
-                                     c)
+    dgate = moe.combine_bwd_gate(bufs.yc, dy, g.index, g.pos, gate_v, s, g_l, c)
     nat.moe_scatter_rows(dy, g.slot_token, g.index.reshape(2, -1).contiguous(),
                          gate_v, ex.peer_dye, ex.e_local, ex.rank, ex.ep)
     ex._Sync(bufs, 2)
@@ -340,8 +311,8 @@ class _MoeFn(torch.autograd.Function):
     # layer's xe/h/dye on this rank has been issued before it in stream order.
     gemm.gemm(dh, wi, True, True, row_ptrs=ex.row_ptrs_dxc)
     ex._Sync(bufs, 3)
-    dx = nat.moe_gather_rows(ex.dxc, g.index, g.pos, gate3, s, g_l, c)
-    return dx, dgate.view_as(gate_v), dwi, dwo, None, None, None, None, None
+    dx = moe.gather_rows(ex.dxc, g.index, g.pos, gate_v, s, g_l, c)
+    return dx, dgate, dwi, dwo, None, None, None, None, None
 
 
 _LOCAL: Dict[int, MoeExchange] = {}
