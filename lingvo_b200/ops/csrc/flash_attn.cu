@@ -72,6 +72,9 @@ __device__ __forceinline__ int lds_s32(uint32_t a) {
 __device__ __forceinline__ void sts_f32(uint32_t a, float v) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory");
 }
+__device__ __forceinline__ void sts_f32x2(uint32_t a, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory");
+}
 __device__ __forceinline__ void sts_s32(uint32_t a, int v) {
   asm volatile("st.shared.s32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
 }
@@ -358,8 +361,13 @@ constexpr int kJChunk = 8;
 constexpr int kBwdMinCtas = 512;
 
 constexpr int kBwdStages = 2;
-// K, V resident + 2 x (Q, dO) + one [128 keys x 64 queries] P/dS tile + barriers / tables.
-constexpr size_t kBwdSmem = kTile * (2 + 2 * kBwdStages) + kChunk + 8192 + 1024;
+// Once the dK / dQ products have read it, the P/dS tile holds the folded fp32 dS^T of the
+// half block for the dRel diagonal sums: [64 rows x 72 columns] (see flash_bwd_kernel).
+constexpr int kDiagCols = 72;
+constexpr int kPdsBytes = 64 * kDiagCols * 4;
+static_assert(kPdsBytes >= kChunk, "the P/dS tile must hold one [128 x 64] bf16 chunk");
+// K, V resident + 2 x (Q, dO) + the P/dS tile + barriers / tables.
+constexpr size_t kBwdSmem = kTile * (2 + 2 * kBwdStages) + kPdsBytes + 8192 + 1024;
 
 // CTA = (key block, h, b); warpgroup g owns keys [64g, 64g + 64) and keeps dK, dV for them in
 // registers. Every visible query block is processed as two 64-row halves (FlashAttention-2
@@ -395,7 +403,7 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
   const uint32_t s_v = s_k + kTile;
   const uint32_t s_qdo = s_v + kTile;                        // stage s: Q at +2s·kTile, dO behind it
   const uint32_t s_pds = s_qdo + 2 * kBwdStages * kTile;     // [128 keys x 64 queries], one chunk
-  uint8_t* meta = smem + kTile * (2 + 2 * kBwdStages) + kChunk;
+  uint8_t* meta = smem + kTile * (2 + 2 * kBwdStages) + kPdsBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(meta);
   uint64_t* kv_bar = bars;
   uint64_t* full_bar = bars + 1;
@@ -515,17 +523,24 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
 #pragma unroll
       for (int n = 0; n < 8; ++n) {
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
+        for (int j = 0; j < 2; ++j) {
+          // The column's tables are read once for both of the thread's key rows.
+          const int qc = hq * 64 + n * 8 + cq + j;   // query column in the tile
+          const float lse_c = lds_f32(s_lse + qc * 4), dlt_c = lds_f32(s_dlt + qc * 4);
+          int seg_c = 1, pos_c = 0;
+          if (!full) {
+            seg_c = lds_s32(s_seg + qc * 4);
+            pos_c = lds_s32(s_pos + qc * 4);
+          }
 #pragma unroll
-          for (int j = 0; j < 2; ++j) {
+          for (int i = 0; i < 2; ++i) {
             const int e = 4 * n + 2 * i + j;
             const int kr = wg * 64 + w16 + 8 * i;    // key row in the tile
-            const int qc = hq * 64 + n * 8 + cq + j; // query column in the tile
             const float x = fmaf(st[e], sl2, lds_f32(s_rel + (qc - kr + 127) * 4));
-            const bool vis = full || ((lds_s32(s_seg + qc * 4) == segk[i]) && (segk[i] != 0) &&
-                                      (!p.mask.causal || lds_s32(s_pos + qc * 4) >= posk[i]));
-            const float pr = vis ? ex2(x - lds_f32(s_lse + qc * 4)) : 0.f;
-            const float ds = pr * (dpt[e] - lds_f32(s_dlt + qc * 4));
+            const bool vis = full || ((seg_c == segk[i]) && (segk[i] != 0) &&
+                                      (!p.mask.causal || pos_c >= posk[i]));
+            const float pr = vis ? ex2(x - lse_c) : 0.f;
+            const float ds = pr * (dpt[e] - dlt_c);
             st[e] = pr;
             dpt[e] = ds;
           }
@@ -579,30 +594,42 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
           *reinterpret_cast<float2*>(dst + n * 8) = make_float2(dq[4 * n + 2 * i], dq[4 * n + 2 * i + 1]);
       }
       if (p.drel_part != nullptr) {
-        // Fixed-order diagonal sums: each warpgroup's [64 keys x 64 queries] fp32 slab goes
-        // through the free P/dS tile; thread t < 127 sums diagonal (query - key) = t - 63.
-#pragma unroll 1
-        for (int sg = 0; sg < 2; ++sg) {
-          named_bar_sync(1, kConsumers);           // every MMA has left the tile / slab consumed
-          if (wg == sg) {
+        // Fixed-order diagonal sums of this half's unrounded fp32 dS^T [128 keys x 64
+        // queries], in one round through the free P/dS tile. A thread's rows k and k + 8 meet
+        // the same diagonals 8 columns apart, so it first adds (n, i = 0) and (n + 1, i = 1)
+        // in registers: row 8w + r of the folded slab is key 16w + r of warp w, and its column
+        // 8 + c holds query column c = -8..63 of that key's diagonals (c - key). The row
+        // stride of 72 floats keeps both the float2 stores and the diagonal reads free of
+        // bank conflicts. Thread t < 191 then sums diagonal (query - key) = t - 127 over the
+        // 64 rows, in four interleaved chains combined in a fixed order.
+        named_bar_sync(1, kConsumers);             // every MMA has left the tile
+        {
+          const uint32_t row = s_pds + (warp_idx * 8 + (lane >> 2)) * (kDiagCols * 4);
 #pragma unroll
-            for (int n = 0; n < 8; ++n)
+          for (int m = -1; m < 8; ++m) {
+            float x[2];
 #pragma unroll
-              for (int i = 0; i < 2; ++i)
-#pragma unroll
-                for (int j = 0; j < 2; ++j)
-                  sts_f32(s_pds + ((w16 + 8 * i) * 64 + n * 8 + cq + j) * 4, dpt[4 * n + 2 * i + j]);
+            for (int j = 0; j < 2; ++j) {
+              x[j] = m >= 0 ? dpt[4 * m + j] : 0.f;
+              if (m < 7) x[j] += dpt[4 * (m + 1) + 2 + j];
+            }
+            sts_f32x2(row + (8 * (m + 1) + cq) * 4, x[0], x[1]);
           }
-          named_bar_sync(1, kConsumers);
-          const int t = threadIdx.x;
-          if (t < 127) {
-            const int dl = t - 63;
-            float sum = 0.f;
-            for (int kl = max(0, -dl); kl < min(64, 64 - dl); ++kl)
-              sum += lds_f32(s_pds + (kl * 64 + kl + dl) * 4);
-            const uint32_t a = s_diag + (dl + 64 * (hq - sg) + 127) * 4;
-            sts_f32(a, lds_f32(a) + sum);
+        }
+        named_bar_sync(1, kConsumers);
+        const int t = threadIdx.x;
+        if (t < 191) {
+          const int dl = t - 127;
+          float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+          for (int rho = 0; rho < 64; ++rho) {
+            const int col = dl + (rho >> 3) * 16 + (rho & 7) + 8;
+            const bool in = col >= 0 && col < kDiagCols;
+            const float x = lds_f32(s_pds + (rho * kDiagCols + (in ? col : 0)) * 4);
+            acc[rho & 3] += in ? x : 0.f;
           }
+          const uint32_t a = s_diag + (hq * 64 + dl + 127) * 4;
+          sts_f32(a, lds_f32(a) + ((acc[0] + acc[1]) + (acc[2] + acc[3])));
         }
       }
     }
@@ -694,9 +721,13 @@ flash_delta_kernel(const __nv_bfloat16* __restrict__ d_o, const __nv_bfloat16* _
 }
 
 // dq_acc[b, l, h, :] += Σ over the launch's key blocks j visible from l's block, in order of j.
+// When the launch covers every key block (dq_acc == nullptr) the sum starts from 0 and goes
+// straight to the bf16 dq, which is what accumulating into a zeroed dq_acc and casting it
+// would give, without the fp32 round trip.
 __global__ void __launch_bounds__(256)
-flash_dq_reduce_kernel(const float4* __restrict__ part, float4* __restrict__ dq_acc, MaskInfo mask,
-                       int B, int L, int H, int j_begin, int jc) {
+flash_dq_reduce_kernel(const float4* __restrict__ part, float4* __restrict__ dq_acc,
+                       uint2* __restrict__ dq, MaskInfo mask, int B, int L, int H, int j_begin,
+                       int jc) {
   const long long n4 = static_cast<long long>(B) * L * H * (kD / 4);
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (idx >= n4) return;
@@ -704,13 +735,16 @@ flash_dq_reduce_kernel(const float4* __restrict__ part, float4* __restrict__ dq_
   const int b = static_cast<int>(row / L);
   const int nblk = L / kT;
   const int4 qm = block_meta(mask, b, nblk, static_cast<int>(row % L) / kT);
-  float4 acc = dq_acc[idx];
+  float4 acc = dq_acc != nullptr ? dq_acc[idx] : make_float4(0.f, 0.f, 0.f, 0.f);
   for (int jr = 0; jr < jc; ++jr) {
     if (!pair_visible(mask, qm, block_meta(mask, b, nblk, j_begin + jr))) continue;
     const float4 v = part[static_cast<long long>(jr) * n4 + idx];
     acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
   }
-  dq_acc[idx] = acc;
+  if (dq_acc != nullptr)
+    dq_acc[idx] = acc;
+  else
+    dq[idx] = make_uint2(pack_bf16x2(acc.x, acc.y), pack_bf16x2(acc.z, acc.w));
 }
 
 // drel[h, t] += Σ_b Σ_j drel_part[b, h, j, t], in order of b, then j.
@@ -946,7 +980,15 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
   p.mask.causal = causal ? 1 : 0;
   auto blk = BlockMeta(p.mask.seg, p.mask.pos, B, L, q.options());
   p.mask.blk = blk.numel() ? reinterpret_cast<const int4*>(blk.data_ptr<int>()) : nullptr;
-  auto dq_acc = torch::zeros({B, L, H, kD}, lse.options());
+  // Key blocks go in launches of up to kJChunk; each launch's per-key-block dQ / dRel partials
+  // are folded in key-block order, so the result does not depend on CTA scheduling. With one
+  // launch the dQ fold writes bf16 dq directly; with several it adds into an fp32 dq_acc.
+  const int nblk = static_cast<int>(L / kT);
+  const int jc_max = nblk < kJChunk ? nblk : kJChunk;
+  const bool one_launch = jc_max == nblk;
+  auto dq = torch::empty({B, L, H, kD}, q.options());
+  torch::Tensor dq_acc;
+  if (!one_launch) dq_acc = torch::zeros({B, L, H, kD}, lse.options());
   auto dk = torch::empty({B, L, Hk, kD}, q.options());
   auto dv = torch::empty({B, L, Hk, kD}, q.options());
   // S > 1: every CTA writes its key block's rows of its run's slice, so no zero-fill is needed.
@@ -974,10 +1016,6 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
                                         static_cast<int>(kBwdSmem)));
     configured = true;
   }
-  // Key blocks go in launches of up to kJChunk; each launch's per-key-block dQ / dRel partials
-  // are folded in key-block order, so the result does not depend on CTA scheduling.
-  const int nblk = static_cast<int>(L / kT);
-  const int jc_max = nblk < kJChunk ? nblk : kJChunk;
   auto dq_part = torch::empty({jc_max, B, L, H, kD}, lse.options());
   p.dq_part = dq_part.data_ptr<float>();
   for (int j_begin = 0; j_begin < nblk; j_begin += jc_max) {
@@ -995,8 +1033,10 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
     C10_CUDA_KERNEL_LAUNCH_CHECK();
     const long long n4 = B * L * H * (kD / 4);
     flash_dq_reduce_kernel<<<static_cast<int>((n4 + 255) / 256), 256, 0, stream>>>(
-        reinterpret_cast<const float4*>(p.dq_part), reinterpret_cast<float4*>(dq_acc.data_ptr<float>()),
-        p.mask, p.B, p.L, p.H, j_begin, jc);
+        reinterpret_cast<const float4*>(p.dq_part),
+        one_launch ? nullptr : reinterpret_cast<float4*>(dq_acc.data_ptr<float>()),
+        one_launch ? reinterpret_cast<uint2*>(dq.data_ptr()) : nullptr, p.mask, p.B, p.L, p.H,
+        j_begin, jc);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
     CountLaunch(2);
     if (need_drel) {
@@ -1016,8 +1056,7 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
     C10_CUDA_KERNEL_LAUNCH_CHECK();
     CountLaunch();
   }
-  auto dq = torch::empty({B, L, H, kD}, q.options());
-  {
+  if (!one_launch) {
     const long long n4 = dq.numel() / 4;
     const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
     long long blocks = (n4 + 255) / 256;
