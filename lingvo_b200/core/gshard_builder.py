@@ -492,15 +492,16 @@ class SelfAttentionLayer(_BuilderLayer):
     simple = (not b.atten_logit_cap) and b.attention_extra_logit is None
     drop = b.attention_dropout_prob if not self.do_eval else 0.0
     toeplitz = (not self.params.relative_bias) or b.relative_attention_use_universal_1d_position
-    if simple and toeplitz:
+    if toeplitz:
       from lingvo_b200.ops import attention as attention_ops
       if attention_ops.flash_attention_supported(q, k, drop):
-        # Our wgmma flash attention: bias table + packed-input mask applied in registers,
-        # dRel folded into the backward; grouped / multi-query KV heads are read in place;
-        # output already `[B, L, H, D]`.
+        # Our wgmma flash attention: bias table + packed-input mask applied in registers (after
+        # the logit cap), dRel folded into the backward; grouped / multi-query KV heads are
+        # read in place; output already `[B, L, H, D]`.
         rel = self._RelTable(theta, l, x.device) if self.params.relative_bias else None
         causal = self.params.decoder and not b.decoder_skip_causal_mask
-        o = attention_ops.flash_attention(q, k, v, rel, segment_id, segment_pos, 1.0, causal)
+        o = attention_ops.flash_attention(q, k, v, rel, segment_id, segment_pos, 1.0, causal,
+                                          **_LogitOptions(b))
         out = gemm.linear(o.reshape(bsz, l, h * d), wo.to(x.dtype), residual=residual)
         return out, torch.zeros((), device=x.device, dtype=torch.float32)
     bias = self._Bias(theta, segment_id, segment_pos,
@@ -547,19 +548,29 @@ def _SelfAttentionExtendStep(layer, theta, x, cache, t):
   if b.use_rotary_position_emb or (layer.params.multi_dconv_head and b.mdha_rope):
     pos = tt.reshape(1, 1).expand(bsz, 1)
     q, k = _Rope(q, pos, b.rope_emb_max_timescale), _Rope(k, pos, b.rope_emb_max_timescale)
-  if b.atten_logit_cap:
-    o = _CappedDecodeAttention(layer, theta, q, k, v, cache, tt)
-  else:
-    # Fused cache append + attention over the live keys (our split-KV kernel on the GPU).
-    from lingvo_b200.ops import attention as attention_ops
-    rel = _DecodeRelTable(layer, theta, tmax, dev)
-    o = attention_ops.decode_attention(q, k, v, cache.k, cache.v, tt, rel)
-    o = o.reshape(bsz, 1, h * d)
+  # Fused cache append + attention over the live keys (our split-KV kernel on the GPU; the
+  # fp32 step of `decode_attention_ref`, in the forward's order, with a cap or extra logit).
+  from lingvo_b200.ops import attention as attention_ops
+  rel = _DecodeRelTable(layer, theta, tmax, dev)
+  o = attention_ops.decode_attention(q, k, v, cache.k, cache.v, tt, rel, **_LogitOptions(b))
+  o = o.reshape(bsz, 1, h * d)
   out = torch.matmul(o, theta.wo.to(xd))
   if layer._tp is not None:   # pylint: disable=protected-access
     from lingvo_b200.parallel import tp_layers   # pylint: disable=g-import-not-at-top
     out = tp_layers.ReduceFromTensorParallel(out, layer._tp)   # pylint: disable=protected-access
   return out
+
+
+def _LogitOptions(b):
+  """The builder's `atten_logit_cap` / `attention_extra_logit` as the keyword arguments of the
+  attention ops, only those that are set: a layer without them calls the ops exactly as
+  before they existed, so wrappers written against the plain signatures keep working."""
+  opts = {}
+  if b.atten_logit_cap:
+    opts['logit_cap'] = float(b.atten_logit_cap)
+  if b.attention_extra_logit is not None:
+    opts['extra_logit'] = float(b.attention_extra_logit)
+  return opts
 
 
 def _DecodeRelTable(layer, theta, tmax, dev):
@@ -599,15 +610,15 @@ def _SelfAttentionPrefill(layer, theta, x, segment_id, segment_pos, cache):
   cache.v[:, :plen] = v.to(cache.v.dtype)
   cache.pos[:, :plen] = segment_pos.to(cache.pos.dtype)
   from lingvo_b200.ops import attention as attention_ops
-  simple = (not b.atten_logit_cap) and b.attention_extra_logit is None
   toeplitz = (not layer.params.relative_bias) or b.relative_attention_use_universal_1d_position
   causal = layer.params.decoder and not b.decoder_skip_causal_mask
   pad = -plen % 128
   padded = [F.pad(t, (0, 0, 0, 0, 0, pad)) for t in (q, k, v)]
-  if simple and toeplitz and attention_ops.flash_attention_supported(padded[0], padded[1]):
+  if toeplitz and attention_ops.flash_attention_supported(padded[0], padded[1]):
     rel = layer._RelTable(theta, plen + pad, x.device) if layer.params.relative_bias else None   # pylint: disable=protected-access
     o = attention_ops.flash_attention(*padded, rel, F.pad(segment_id, (0, pad)),
-                                      F.pad(segment_pos, (0, pad)), 1.0, causal)[:, :plen]
+                                      F.pad(segment_pos, (0, pad)), 1.0, causal,
+                                      **_LogitOptions(b))[:, :plen]
   else:
     bias = layer._Bias(theta, segment_id, segment_pos, torch.float32)   # pylint: disable=protected-access
     o = _AttentionCore(q, k, v, bias, b.atten_logit_cap, b.attention_extra_logit)
@@ -634,38 +645,9 @@ def _SelfAttentionBeamStep(layer, theta, x, cache, slot0, vis, qpos):
   from lingvo_b200.ops import attention as attention_ops
   o = attention_ops.flat_beam_attention(
       q, k, v, cache.k, cache.v, slot0, vis, qpos, cache.pos,
-      _DecodeRelTable(layer, theta, tmax, x.device), 1.0, b.atten_logit_cap)
+      _DecodeRelTable(layer, theta, tmax, x.device), 1.0, b.atten_logit_cap,
+      b.attention_extra_logit)
   return _SelfAttentionOut(layer, theta, o.reshape(bsz, kk, h * d), xd)
-
-
-def _CappedDecodeAttention(layer, theta, q, k, v, cache, tt):
-  """Decode-step attention of a layer with `atten_logit_cap`: one-hot cache write, fp32 logits
-  over every cached key, the cap applied to q·k + bias − 1e9·future. Returns `[B,1,H·D]`."""
-  b = layer.bp
-  bsz, _, h, d = q.shape
-  hk = k.shape[2]
-  xd = q.dtype
-  tmax = cache.k.shape[1]
-  dev = q.device
-  onehot = (torch.arange(tmax, device=dev) == tt).to(xd).reshape(1, tmax, 1, 1)
-  cache.k.mul_(1 - onehot).add_(k * onehot)
-  cache.v.mul_(1 - onehot).add_(v * onehot)
-  kk, vv = cache.k, cache.v
-  if hk != h:
-    kk, vv = kk.expand(bsz, tmax, h, d), vv.expand(bsz, tmax, h, d)
-  logits = torch.einsum('bqhd,bkhd->bhqk', q.float(), kk.float())      # [B,H,1,T]
-  key_pos = torch.arange(tmax, device=dev)
-  if layer.params.relative_bias:
-    bucket = RelativePositionBucket(
-        key_pos - tt, b.relative_attention_num_buckets, b.relative_attention_max_distance,
-        bidirectional=b.decoder_bidirectional_relative_attention)
-    logits = logits + theta.wrb.float()[:, bucket.long()].reshape(1, h, 1, tmax)
-  logits = logits + ((key_pos > tt).float() * -1e9).reshape(1, 1, 1, tmax)
-  if b.atten_logit_cap:
-    logits = b.atten_logit_cap * torch.tanh(logits / b.atten_logit_cap)
-  probs = torch.softmax(logits, -1)
-  o = torch.einsum('bhqk,bkhd->bqhd', probs, vv.float()).to(xd).reshape(bsz, 1, h * d)
-  return o
 
 
 def _Rope(x, pos, max_timescale):

@@ -92,6 +92,7 @@ class DenseLmTemplate(base_model_params.SingleTaskModelParams):
   DEVICE_MESH = None
   DEBUG = False
   ATTEN_LOGIT_CAP = 0
+  ATTENTION_EXTRA_LOGIT = None
   MODEL_DIM_RESHAPE_SEGMENTS = None
   GATED_GELU = True
   POSITIONAL_EMBEDDING = False
@@ -113,7 +114,7 @@ class DenseLmTemplate(base_model_params.SingleTaskModelParams):
         num_devices=1,
         attention_dropout_prob=0.0,
         attention_key_value_dim=self.ATTENTION_KEY_VALUE_DIM,
-        attention_extra_logit=None,
+        attention_extra_logit=self.ATTENTION_EXTRA_LOGIT,
         relative_attention_use_universal_1d_position=True,
         model_dim_reshape_segments=self.MODEL_DIM_RESHAPE_SEGMENTS,
         model_dim=self.MODEL_DIM,
@@ -461,6 +462,15 @@ class MoELm8EKv4(MoELm8E):
   """MoELm8E with grouped-query attention: 16 query heads share 4 KV heads (wk, wv
   [2048, 512]), which makes the decoding KV cache 4x smaller."""
   NUM_KV_HEADS = 4
+
+
+@model_registry.RegisterSingleTaskModel
+class MoELm8ESoftCap(MoELm8E):
+  """MoELm8E with the reference's attention options: the logits soft-capped at 50
+  (cap·tanh(q·k / cap), before the relative bias) and an extra logit of 0 in every softmax.
+  Both run inside our flash attention kernels."""
+  ATTEN_LOGIT_CAP = 50.0
+  ATTENTION_EXTRA_LOGIT = 0.0
 
 
 @model_registry.RegisterSingleTaskModel

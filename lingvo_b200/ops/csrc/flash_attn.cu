@@ -19,6 +19,16 @@
 // head h reads KV head h / G, G = H / Hk (the convention of `_ExpandKv` and decode_attn.cu).
 // With Hk == H every kernel does exactly what the multi-head kernels did.
 //
+// Soft-capped logits and an extra logit (GShard `atten_logit_cap`, `attention_extra_logit`):
+//
+//   z_ij = cap·tanh(scale·q_i·k_j / cap) + rel[h, i-j+L-1] + mask(b,i,j)
+//   O_i  = Σ_j softmax(z_i ∪ {extra})_j · v_j      (the extra slot has value 0)
+//
+// The cap applies to scale·q·k only; the bias and the mask are added after it. Both are
+// compile-time specialisations (flash_fwd_kernel<kCap, kExtra>, flash_bwd_kernel<kCap>), so the
+// default instantiations are the plain kernels. The extra logit needs no backward code: lse
+// already counts it and delta = Σ dO∘O is right because the extra slot's value is 0.
+//
 // Layouts: q, dO [B, L, H, D=128] and k, v [B, L, Hk, D] bf16 views (strides (*, *, D, 1));
 // O [B, L, H, D] and dK, dV [B, L, Hk, D] contiguous bf16;  dq_part [Jc, B, L, H, D] fp32;
 // dk_part, dv_part [S, B, L, Hk, D] fp32 (only when the group is split, S > 1);  lse, delta
@@ -56,6 +66,18 @@ __device__ __forceinline__ float lg2(float x) {
   float y;
   asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
+}
+__device__ __forceinline__ float rcp(float x) {
+  float y;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+// tanh(u) = 1 - 2r with r = 1 / (1 + e^{2u}), from a = 2u·log2e: one ex2 and one reciprocal,
+// with an absolute error near fp32 rounding for every u (tanh.approx.f32 is only good to about
+// 2^-11 relative, which a logit near a cap of 50 would feel). 1 - tanh(u)^2 = 4r(1 - r).
+__device__ __forceinline__ float tanh_r(float a, float& r) {
+  r = rcp(1.f + ex2(a));
+  return fmaf(-2.f, r, 1.f);
 }
 // Explicit shared-space accesses: the tile base is re-aligned through integer arithmetic,
 // after which the compiler can only emit *generic* LD/ST for C++ pointers into it.
@@ -133,6 +155,10 @@ struct FwdParams {
   int B, H, L;
   int G;                 // query heads per KV head
   float scale;
+  float cap_l2;          // kCap: cap·log2e
+  float cap_a;           // kCap: 2·scale·log2e / cap, so that tanh(scale·s / cap) = tanh_r(s·cap_a)
+  float extra_l2;        // kExtra: extra·log2e
+  float extra;           // kExtra: the extra logit
 };
 
 // smem: Q | (K, V) x 2 stages | P x 2 warpgroups (16 KiB each) + barriers / per-block tables.
@@ -142,6 +168,7 @@ constexpr size_t kFwdSmem = kTile * 6 + 4096 + 1024;
 //   S = Q·K^T (wgmma, registers) | online softmax | P (bf16) -> smem | O += P·V (wgmma)
 // on its 64 query rows. CTA = (query block, query head h, b); K/V come from KV head h / G.
 // The heads of a group are adjacent in blockIdx.y, so their K/V tiles are re-read from L2.
+template <bool kCap, bool kExtra>
 __global__ void __launch_bounds__(kThreads, 1)
 flash_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                  const __grid_constant__ CUtensorMap map_v, const FwdParams p) {
@@ -221,7 +248,10 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
   float o[64];
 #pragma unroll
   for (int c = 0; c < 64; ++c) o[c] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  // With an extra logit the running max starts at it: exp(extra - m) then stays <= 1 and is
+  // added to l at the end, and a row that sees nothing keeps m = extra, l = 0.
+  const float m0 = kExtra ? p.extra_l2 : -INFINITY;
+  float m_run[2] = {m0, m0}, l_run[2] = {0.f, 0.f};
   mbar_wait(smem_u32(q_bar), 0);
 
   int it = 0;
@@ -268,7 +298,13 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
         for (int j = 0; j < 2; ++j) {
           const int r = wg * 64 + pr0 + 8 * i;       // query row in the tile
           const int c = n * 8 + cq + j;              // key column in the tile
-          float x = fmaf(sv[4 * n + 2 * i + j], sl2, lds_f32(s_rel + (r - c + 127) * 4));
+          float x;
+          if constexpr (kCap) {
+            float rr;
+            x = fmaf(p.cap_l2, tanh_r(sv[4 * n + 2 * i + j] * p.cap_a, rr), lds_f32(s_rel + (r - c + 127) * 4));
+          } else {
+            x = fmaf(sv[4 * n + 2 * i + j], sl2, lds_f32(s_rel + (r - c + 127) * 4));
+          }
           if (!full) {
             const bool vis = (segq[i] == lds_s32(s_seg + c * 4)) && (segq[i] != 0) &&
                              (!p.mask.causal || posq[i] >= lds_s32(s_pos + c * 4));
@@ -323,6 +359,7 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
     float l = l_run[i];
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
+    if constexpr (kExtra) l += ex2(p.extra_l2 - m_run[i]);   // >= 1 when the row sees nothing
     const float inv = l > 0.f ? 1.f / l : 0.f;      // query block that sees nothing: 0
     const int qi = i0 + wg * 64 + pr0 + 8 * i;
     __nv_bfloat16* dst = p.out + ((bl + qi) * p.H + h) * kD;
@@ -330,9 +367,12 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
     for (int n = 0; n < 16; ++n)
       *reinterpret_cast<uint32_t*>(dst + n * 8 + cq) =
           pack_bf16x2(o[4 * n + 2 * i] * inv, o[4 * n + 2 * i + 1] * inv);
+    // With an extra logit, relative to it, so that a row that sees nothing (m = extra, l = 1)
+    // gets lse == extra exactly.
     if ((lane & 3) == 0)
       p.lse[(static_cast<long long>(b) * p.H + h) * p.L + qi] =
-          l > 0.f ? (m_run[i] + lg2(l)) * kLn2 : 0.f;
+          kExtra ? fmaf((m_run[i] - p.extra_l2) + lg2(l), kLn2, p.extra)
+                 : (l > 0.f ? (m_run[i] + lg2(l)) * kLn2 : 0.f);
   }
 }
 
@@ -352,6 +392,7 @@ struct BwdParams {
   int Hk, G, S;          // KV heads, query heads per KV head, runs per group
   int j_begin, jc;       // this launch covers key blocks [j_begin, j_begin + jc)
   float scale;
+  float cap_l2, cap_a;   // kCap: as in FwdParams
 };
 
 // Key blocks per backward launch (the leading dimension of dq_part / drel_part).
@@ -382,6 +423,10 @@ constexpr size_t kBwdSmem = kTile * (2 + 2 * kBwdStages) + kPdsBytes + 8192 + 10
 // as this run's slice of dk_part / dv_part, folded in run order by flash_dkv_fold_kernel.
 // No atomics: the partials are folded in key-block order by the reduce kernels below, so
 // the gradients are identical run to run.
+// kCap: z = cap·tanh(s/cap) + rel, so dRel takes dS and dQ / dK take dS∘(1 - t²). P^T goes to
+// the P/dS tile inside the element loop, which frees st[] to carry scale·(1 - t²) to the dS^T
+// store while dpt[] keeps the plain dS for the diagonal sums: no third 32-float array.
+template <bool kCap>
 __global__ void __launch_bounds__(kThreads, 1)
 flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                  const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do,
@@ -522,6 +567,7 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
       wgmma_fence_regs(dpt);
 #pragma unroll
       for (int n = 0; n < 8; ++n) {
+        float pv[2][2];        // kCap: P^T of the thread's (row i, column j) at this n
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
           // The column's tables are read once for both of the thread's key rows.
@@ -536,22 +582,39 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
           for (int i = 0; i < 2; ++i) {
             const int e = 4 * n + 2 * i + j;
             const int kr = wg * 64 + w16 + 8 * i;    // key row in the tile
-            const float x = fmaf(st[e], sl2, lds_f32(s_rel + (qc - kr + 127) * 4));
+            float x, rr = 0.f;
+            if constexpr (kCap)
+              x = fmaf(p.cap_l2, tanh_r(st[e] * p.cap_a, rr), lds_f32(s_rel + (qc - kr + 127) * 4));
+            else
+              x = fmaf(st[e], sl2, lds_f32(s_rel + (qc - kr + 127) * 4));
             const bool vis = full || ((seg_c == segk[i]) && (segk[i] != 0) &&
                                       (!p.mask.causal || pos_c >= posk[i]));
             const float pr = vis ? ex2(x - lse_c) : 0.f;
             const float ds = pr * (dpt[e] - dlt_c);
-            st[e] = pr;
+            if constexpr (kCap) {
+              pv[i][j] = pr;
+              st[e] = (4.f * rr) * (1.f - rr) * p.scale;   // scale·(1 - t²)
+            } else {
+              st[e] = pr;
+            }
             dpt[e] = ds;
           }
         }
+        if constexpr (kCap) {
+#pragma unroll
+          for (int i = 0; i < 2; ++i)
+            sts_b32(s_pds + sw128_off(wg * 64 + w16 + 8 * i, n * 8 + cq, kChunk),
+                    pack_bf16x2(pv[i][0], pv[i][1]));
+        }
       }
+      if constexpr (!kCap) {
 #pragma unroll
-      for (int n = 0; n < 8; ++n)
+        for (int n = 0; n < 8; ++n)
 #pragma unroll
-        for (int i = 0; i < 2; ++i)
-          sts_b32(s_pds + sw128_off(wg * 64 + w16 + 8 * i, n * 8 + cq, kChunk),
-                  pack_bf16x2(st[4 * n + 2 * i], st[4 * n + 2 * i + 1]));
+          for (int i = 0; i < 2; ++i)
+            sts_b32(s_pds + sw128_off(wg * 64 + w16 + 8 * i, n * 8 + cq, kChunk),
+                    pack_bf16x2(st[4 * n + 2 * i], st[4 * n + 2 * i + 1]));
+      }
       fence_proxy_async();
       named_bar_sync(2 + wg, 128);
       wgmma_fence();
@@ -566,9 +629,15 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
 #pragma unroll
       for (int n = 0; n < 8; ++n)
 #pragma unroll
-        for (int i = 0; i < 2; ++i)
-          sts_b32(s_pds + sw128_off(wg * 64 + w16 + 8 * i, n * 8 + cq, kChunk),
-                  pack_bf16x2(dpt[4 * n + 2 * i] * p.scale, dpt[4 * n + 2 * i + 1] * p.scale));
+        for (int i = 0; i < 2; ++i) {
+          const int e = 4 * n + 2 * i;
+          if constexpr (kCap)
+            sts_b32(s_pds + sw128_off(wg * 64 + w16 + 8 * i, n * 8 + cq, kChunk),
+                    pack_bf16x2(dpt[e] * st[e], dpt[e + 1] * st[e + 1]));
+          else
+            sts_b32(s_pds + sw128_off(wg * 64 + w16 + 8 * i, n * 8 + cq, kChunk),
+                    pack_bf16x2(dpt[e] * p.scale, dpt[e + 1] * p.scale));
+        }
       fence_proxy_async();
       named_bar_sync(1, kConsumers);               // dQ reads every key row of dS^T
       float dq[32];            // written by the first dQ MMA (scale-d = 0)
@@ -876,6 +945,43 @@ torch::Tensor BlockMeta(const int* seg, const int* pos, int64_t B, int64_t L,
   return out;
 }
 
+// A negative or non-finite cap, or a non-finite extra logit, is refused before anything is
+// allocated or launched.
+void CheckLogitOptions(const char* op, double logit_cap, const c10::optional<double>& extra_logit) {
+  TORCH_CHECK(std::isfinite(logit_cap) && logit_cap >= 0.0, op,
+              ": logit_cap must be finite and >= 0 (0 = no cap), got ", logit_cap);
+  TORCH_CHECK(!extra_logit.has_value() || std::isfinite(*extra_logit), op,
+              ": extra_logit must be finite, got ", extra_logit.value_or(0.0));
+}
+
+// One launch of an instantiation; each instantiation sets its own dynamic shared-memory limit
+// the first time it is launched.
+template <bool kCap, bool kExtra>
+void LaunchFwd(dim3 grid, cudaStream_t stream, const CUtensorMap& mq, const CUtensorMap& mk,
+               const CUtensorMap& mv, const FwdParams& p) {
+  static bool configured = false;
+  if (!configured) {
+    C10_CUDA_CHECK(cudaFuncSetAttribute(flash_fwd_kernel<kCap, kExtra>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        static_cast<int>(kFwdSmem)));
+    configured = true;
+  }
+  flash_fwd_kernel<kCap, kExtra><<<grid, kThreads, kFwdSmem, stream>>>(mq, mk, mv, p);
+}
+
+template <bool kCap>
+void LaunchBwd(dim3 grid, cudaStream_t stream, const CUtensorMap& mq, const CUtensorMap& mk,
+               const CUtensorMap& mv, const CUtensorMap& mdo, const BwdParams& p) {
+  static bool configured = false;
+  if (!configured) {
+    C10_CUDA_CHECK(cudaFuncSetAttribute(flash_bwd_kernel<kCap>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        static_cast<int>(kBwdSmem)));
+    configured = true;
+  }
+  flash_bwd_kernel<kCap><<<grid, kThreads, kBwdSmem, stream>>>(mq, mk, mv, mdo, p);
+}
+
 }  // namespace
 
 // Runs S into which the backward splits each group of G = H / Hk query heads: the smallest
@@ -892,14 +998,17 @@ int64_t flash_attn_bwd_splits(int64_t B, int64_t L, int64_t H, int64_t Hk) {
   return s;
 }
 
-// Returns (out [B,L,H,D] bf16, lse [B,H,L] fp32).
+// Returns (out [B,L,H,D] bf16, lse [B,H,L] fp32). logit_cap > 0 soft-caps scale·q·k;
+// extra_logit adds one logit of value 0 to every softmax (lse counts it).
 std::vector<torch::Tensor> flash_attn_fwd(const torch::Tensor& q, const torch::Tensor& k,
                                           const torch::Tensor& v,
                                           const c10::optional<torch::Tensor>& rel,
                                           const c10::optional<torch::Tensor>& seg,
                                           const c10::optional<torch::Tensor>& pos, double scale,
-                                          bool causal) {
+                                          bool causal, double logit_cap,
+                                          const c10::optional<double>& extra_logit) {
   CheckArgs("flash_attn_fwd", q, k, v, rel, seg, pos);
+  CheckLogitOptions("flash_attn_fwd", logit_cap, extra_logit);
   const int64_t B = q.size(0), L = q.size(1), H = q.size(2);
   const c10::cuda::CUDAGuard guard(q.device());
   FwdParams p;
@@ -921,32 +1030,41 @@ std::vector<torch::Tensor> flash_attn_fwd(const torch::Tensor& q, const torch::T
   p.B = static_cast<int>(B); p.H = static_cast<int>(H); p.L = static_cast<int>(L);
   p.G = static_cast<int>(H / k.size(2));
   p.scale = static_cast<float>(scale);
+  const bool cap = logit_cap > 0.0, extra = extra_logit.has_value();
+  p.cap_l2 = cap ? static_cast<float>(logit_cap * kLog2e) : 0.f;
+  p.cap_a = cap ? static_cast<float>(2.0 * scale * kLog2e / logit_cap) : 0.f;
+  p.extra = extra ? static_cast<float>(*extra_logit) : 0.f;
+  p.extra_l2 = p.extra * kLog2e;
   auto mk = [&](const torch::Tensor& t) {
     return MakeMap(t.data_ptr(), t.size(2) * kD, L, B, t.stride(1), t.stride(0), kT);
   };
   const CUtensorMap mq = mk(q), mkk = mk(k), mv = mk(v);
-  static bool configured = false;
-  if (!configured) {
-    C10_CUDA_CHECK(cudaFuncSetAttribute(flash_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(kFwdSmem)));
-    configured = true;
-  }
   dim3 grid(static_cast<unsigned>(L / kT), static_cast<unsigned>(H), static_cast<unsigned>(B));
-  flash_fwd_kernel<<<grid, kThreads, kFwdSmem, at::cuda::getCurrentCUDAStream()>>>(mq, mkk, mv, p);
+  auto stream = at::cuda::getCurrentCUDAStream();
+  if (cap && extra)
+    LaunchFwd<true, true>(grid, stream, mq, mkk, mv, p);
+  else if (cap)
+    LaunchFwd<true, false>(grid, stream, mq, mkk, mv, p);
+  else if (extra)
+    LaunchFwd<false, true>(grid, stream, mq, mkk, mv, p);
+  else
+    LaunchFwd<false, false>(grid, stream, mq, mkk, mv, p);
   C10_CUDA_KERNEL_LAUNCH_CHECK();
   CountLaunch();
   return {out, lse};
 }
 
 // Returns (dq [B,L,H,D], dk, dv [B,L,Hk,D] bf16, drel [H,2L-1] fp32 or an empty tensor).
+// logit_cap is the forward's; an extra logit needs nothing here (lse already counts it).
 std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::Tensor& k,
                                           const torch::Tensor& v, const torch::Tensor& out,
                                           const torch::Tensor& d_out, const torch::Tensor& lse,
                                           const c10::optional<torch::Tensor>& rel,
                                           const c10::optional<torch::Tensor>& seg,
                                           const c10::optional<torch::Tensor>& pos, double scale,
-                                          bool causal, bool need_drel) {
+                                          bool causal, bool need_drel, double logit_cap) {
   CheckArgs("flash_attn_bwd", q, k, v, rel, seg, pos, &out, &d_out, &lse);
+  CheckLogitOptions("flash_attn_bwd", logit_cap, c10::nullopt);
   const int64_t B = q.size(0), L = q.size(1), H = q.size(2), Hk = k.size(2);
   const int64_t S = flash_attn_bwd_splits(B, L, H, Hk);
   const c10::cuda::CUDAGuard guard(q.device());
@@ -1006,16 +1124,13 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
   p.B = static_cast<int>(B); p.H = static_cast<int>(H); p.L = static_cast<int>(L);
   p.Hk = static_cast<int>(Hk); p.G = static_cast<int>(H / Hk); p.S = static_cast<int>(S);
   p.scale = static_cast<float>(scale);
+  const bool cap = logit_cap > 0.0;
+  p.cap_l2 = cap ? static_cast<float>(logit_cap * kLog2e) : 0.f;
+  p.cap_a = cap ? static_cast<float>(2.0 * scale * kLog2e / logit_cap) : 0.f;
   auto mk = [&](const torch::Tensor& t) {
     return MakeMap(t.data_ptr(), t.size(2) * kD, L, B, t.stride(1), t.stride(0), kT);
   };
   const CUtensorMap mq = mk(q), mkk = mk(k), mv = mk(v), mdo = mk(d_o);
-  static bool configured = false;
-  if (!configured) {
-    C10_CUDA_CHECK(cudaFuncSetAttribute(flash_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(kBwdSmem)));
-    configured = true;
-  }
   auto dq_part = torch::empty({jc_max, B, L, H, kD}, lse.options());
   p.dq_part = dq_part.data_ptr<float>();
   for (int j_begin = 0; j_begin < nblk; j_begin += jc_max) {
@@ -1029,7 +1144,10 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
       p.drel_part = drel_part.data_ptr<float>();
     }
     dim3 grid(static_cast<unsigned>(jc), static_cast<unsigned>(Hk * S), static_cast<unsigned>(B));
-    flash_bwd_kernel<<<grid, kThreads, kBwdSmem, stream>>>(mq, mkk, mv, mdo, p);
+    if (cap)
+      LaunchBwd<true>(grid, stream, mq, mkk, mv, mdo, p);
+    else
+      LaunchBwd<false>(grid, stream, mq, mkk, mv, mdo, p);
     C10_CUDA_KERNEL_LAUNCH_CHECK();
     const long long n4 = B * L * H * (kD / 4);
     flash_dq_reduce_kernel<<<static_cast<int>((n4 + 255) / 256), 256, 0, stream>>>(
@@ -1074,10 +1192,12 @@ std::vector<torch::Tensor> flash_attn_bwd(const torch::Tensor& q, const torch::T
 
 LB_REGISTER(flash_attn) {
   m.def("flash_attn_fwd", &lb::flash_attn_fwd, py::arg("q"), py::arg("k"), py::arg("v"),
-        py::arg("rel"), py::arg("seg"), py::arg("pos"), py::arg("scale"), py::arg("causal"));
+        py::arg("rel"), py::arg("seg"), py::arg("pos"), py::arg("scale"), py::arg("causal"),
+        py::arg("logit_cap") = 0.0, py::arg("extra_logit") = py::none());
   m.def("flash_attn_bwd", &lb::flash_attn_bwd, py::arg("q"), py::arg("k"), py::arg("v"),
         py::arg("out"), py::arg("d_out"), py::arg("lse"), py::arg("rel"), py::arg("seg"),
-        py::arg("pos"), py::arg("scale"), py::arg("causal"), py::arg("need_drel"));
+        py::arg("pos"), py::arg("scale"), py::arg("causal"), py::arg("need_drel"),
+        py::arg("logit_cap") = 0.0);
   m.def("flash_attn_bwd_splits", &lb::flash_attn_bwd_splits, py::arg("B"), py::arg("L"),
         py::arg("H"), py::arg("Hk"));
 }

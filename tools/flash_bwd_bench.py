@@ -10,6 +10,8 @@ For every Hk:
   * `ms`: CUDA events around `--iters` back-to-back `flash_attn_bwd` calls after warm-up,
     divided by the count. This is the whole entry point: the delta, block-summary, dQ fold,
     dRel fold and dK/dV fold kernels and the allocator's fills are all inside it.
+  * `fwd_ms`, `fwd_bwd_ms`: the same for `flash_attn_fwd` alone and for a forward followed by
+    its backward.
   * `tflops`: the FLOPs of the visible (query block, key block) pairs, counted here from the
     mask (5 products of 2·128^3 per pair and head), over `ms`.
   * `peak_mb`: torch.cuda.max_memory_allocated during one call, above what was allocated
@@ -18,6 +20,10 @@ For every Hk:
     torch.profiler in a separate pass after the timed one.
 The card's name, power limit and SM clock (sampled with nvidia-smi while the timed loop
 runs) go in the same line.
+
+`--cap C` soft-caps the logits at C and `--extra X` adds an extra logit X (the specialised
+kernels of GShard's `atten_logit_cap` / `attention_extra_logit`); without them the calls pass
+neither option, so a checkout that predates them can be timed too.
 
 `--root DIR` imports lingvo_b200 from another checkout (built in place), so two versions can
 be timed alternately in one job.
@@ -35,6 +41,8 @@ def _Args():
   ap.add_argument('--hk', default='16,4,1', help='comma-separated KV head counts')
   ap.add_argument('--iters', type=int, default=100)
   ap.add_argument('--warmup', type=int, default=10)
+  ap.add_argument('--cap', type=float, default=0.0, help='logit_cap (0 = none)')
+  ap.add_argument('--extra', type=float, default=None, help='extra_logit (default none)')
   ap.add_argument('--profile', action='store_true', help='add a torch.profiler kernel split')
   ap.add_argument('--out', default=None, help='also write the JSON line to this file')
   return ap.parse_args()
@@ -122,11 +130,26 @@ def main():
   info = _Smi('name,power.limit,clocks.max.sm') or ['?', '?', '?']
   res = dict(tool='flash_bwd_bench', root=os.path.abspath(ARGS.root), gpu=info[0],
              power_limit_w=info[1], max_sm_clock_mhz=info[2], B=B, L=L, H=H, D=D,
-             causal=True, iters=ARGS.iters, gflop=round(_Flops() / 1e9, 2), cases={})
+             causal=True, logit_cap=ARGS.cap, extra_logit=ARGS.extra, iters=ARGS.iters,
+             gflop=round(_Flops() / 1e9, 2), cases={})
+  fwd_opts, bwd_opts = {}, {}
+  if ARGS.cap:
+    fwd_opts['logit_cap'] = bwd_opts['logit_cap'] = ARGS.cap
+  if ARGS.extra is not None:
+    fwd_opts['extra_logit'] = ARGS.extra
   for hk in [int(x) for x in ARGS.hk.split(',')]:
     q, k, v, rel, seg, pos, d_o = _Inputs(hk)
-    out, lse = nat.flash_attn_fwd(q, k, v, rel, seg, pos, 1.0, True)
-    call = lambda: nat.flash_attn_bwd(q, k, v, out, d_o, lse, rel, seg, pos, 1.0, True, True)
+    fwd = lambda: nat.flash_attn_fwd(q, k, v, rel, seg, pos, 1.0, True, **fwd_opts)
+    out, lse = fwd()
+    call = lambda: nat.flash_attn_bwd(q, k, v, out, d_o, lse, rel, seg, pos, 1.0, True, True,
+                                      **bwd_opts)
+
+    def fwd_bwd():
+      o, l = fwd()
+      return nat.flash_attn_bwd(q, k, v, o, d_o, l, rel, seg, pos, 1.0, True, True, **bwd_opts)
+    for _ in range(ARGS.warmup):
+      fwd()
+      fwd_bwd()
     for _ in range(ARGS.warmup):
       call()
     torch.cuda.synchronize()
@@ -137,7 +160,10 @@ def main():
     peak = torch.cuda.max_memory_allocated() - base
     del grads
     ms, clock = _Time(call, ARGS.iters)
+    fwd_ms, _ = _Time(fwd, ARGS.iters)
+    fwd_bwd_ms, _ = _Time(fwd_bwd, ARGS.iters)
     case = dict(hk=hk, splits=int(nat.flash_attn_bwd_splits(B, L, H, hk)), ms=round(ms, 4),
+                fwd_ms=round(fwd_ms, 4), fwd_bwd_ms=round(fwd_bwd_ms, 4),
                 tflops=round(_Flops() / (ms * 1e-3) / 1e12, 1),
                 peak_mb=round(peak / 2**20, 1), sm_clock_mhz=clock)
     if ARGS.profile:
